@@ -1,4 +1,4 @@
-"""Drop-in alias: `import COTR...` resolves to the B200-native implementation in `cotr_b200`.
+"""Drop-in alias: `import COTR...` resolves to the H100-native implementation in `cotr_b200`.
 
 The reference's demos (e.g. demo_single_pair.py) do
     from COTR.utils import utils, debug_utils

@@ -1,6 +1,6 @@
-"""Benchmark of the COTR correspondence hot path on B200 (contract: see the task statement / DESIGN.md section 6).
+"""Benchmark of the COTR correspondence hot path on H100 (DESIGN.md section 6).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl native|reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl native|reference] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 --master-port P bench.py --gpus N ...
 
 Workload (BASELINE.json configs[1], the one `metric` is quoted on): per GPU one synthetic 256x256 image pair laid side
@@ -24,6 +24,9 @@ One JSON line on rank 0:
   cpu_baseline  the oracle port (CPU restatement of the reference, oracle/cotr_oracle.py) on the host cores, rank 0, N=1
 `--impl reference` times that CPU path alone (all host threads) and prints the same line shape with "impl": "reference".
 `--config 3` / `--config 5` time the zoom-in engines instead (see DESIGN.md section 6).
+`--dump-outputs DIR` writes, after the timed steps, what the last timed step returned (rank 0's (1,1024,2) predicted
+correspondences) as DIR/pred_corrs.npy in float32; weights and inputs are seeded, so two builds run with the same
+arguments can be compared output for output.
 """
 import argparse
 import json
@@ -57,7 +60,7 @@ def measured_peaks():
         with open(path) as f:
             p = json.load(f)
         return {"bf16_tflops": float(p["bf16_tflops"]), "hbm_gbs": float(p["hbm_gbs"]), "source": "measured (MEASURED_PEAKS.json, burst)"}
-    return {"bf16_tflops": 1590.0, "hbm_gbs": 6650.0, "source": "fallback (B200_PROFILING.md)"}
+    return {"bf16_tflops": 989.0, "hbm_gbs": 3350.0, "source": "NVIDIA H100 SXM data sheet (dense BF16, 700 W card)"}
 
 
 class ClockSampler:
@@ -146,8 +149,8 @@ def config_dict(world):
 
 
 def committed_traffic():
-    """dram__bytes_read.sum + dram__bytes_write.sum per launch of the dominant kernel, from the committed
-    `ncu --set full` capture of this round (profiles/r02_traffic.json, written by tools/ncu_summary.py)."""
+    """dram__bytes_read.sum + dram__bytes_write.sum per launch of the dominant kernel, from a committed
+    `ncu --set full` capture (profiles/r02_traffic.json) when one exists for this build."""
     path = os.path.join(REPO, "profiles", "r02_traffic.json")
     try:
         with open(path) as f:
@@ -289,7 +292,7 @@ def run_native(args, rank, local_rank, world):
     q_pin = torch.from_numpy(q_np).pin_memory()
     out_pin = torch.empty((1, N_QUERIES, 2), dtype=torch.float32).pin_memory()
     gathered_pin = torch.empty((world, N_QUERIES, 2), dtype=torch.float32).pin_memory() if world > 1 else None
-    flush = torch.empty(256 * 1024 * 1024, dtype=torch.uint8, device=dev)     # > 126 MB L2
+    flush = torch.empty(256 * 1024 * 1024, dtype=torch.uint8, device=dev)     # > 50 MB L2
 
     from cotr_b200.inference.sharding import AsyncGather
     # N > 1: the 8 KB blocks are exchanged on a side stream - this library's peer-memory push over NVLink on one node, NCCL otherwise
@@ -321,6 +324,7 @@ def run_native(args, rank, local_rank, world):
 
     # ---- value: K steps, each bracketed by CUDA events on the launching stream, L2 flushed between steps ----------
     dev_ms = _timed_steps(step, flush, args.steps, barrier)
+    dumped = last["pred"].detach().float().cpu().numpy()    # the last timed step's result, before anything else runs
     launches_per_step = nat.last_launch_count()
     gather_ok, solo_ms, rank_ms = None, dev_ms, [dev_ms]
     if world > 1:
@@ -375,7 +379,7 @@ def run_native(args, rank, local_rank, world):
     def step4():
         gather4.submit(model(img4, q4)["pred_corrs"])
 
-    c4_steps = max(5, min(args.steps, 20))
+    c4_steps = args.steps
     c4_ms, c4_launches = float("nan"), 0
     if not args.quick:
         for _ in range(3):
@@ -452,7 +456,7 @@ def run_native(args, rank, local_rank, world):
     line = {
         "metric": METRIC, "value": value, "unit": UNIT, "n_gpus": world, "steps": args.steps, "warmup": max(args.warmup, 3),
         "ms_per_step": dev_ms, "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
-        "dtype": "f32 (fp16 hi/lo split operands, fp32 accumulate on tcgen05)", "data": "synthetic",
+        "dtype": "f32 (fp16 hi/lo split operands, fp32 accumulate on wgmma)", "data": "synthetic",
         "config": config_dict(world),
         "e2e": {"value": total_q / (e2e_ms * 1e-3), "unit": UNIT, "ms_per_step": e2e_ms,
                 "h2d_bytes_per_step": int(img_np.nbytes + q_np.nbytes), "d2h_bytes_per_step": d2h, "api": e2e_api},
@@ -478,6 +482,9 @@ def run_native(args, rank, local_rank, world):
         line["roofline"] = None
     if world == 1 and not args.quick:
         line["cpu_baseline"] = cpu_reference_rate(budget_s=10.0)
+    if args.dump_outputs:
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        np.save(os.path.join(args.dump_outputs, "pred_corrs.npy"), dumped.astype(np.float32))
     print(json.dumps(line))
 
 
@@ -491,6 +498,8 @@ def main():
                     help="headline steps only (no configs[3] block, no CPU baseline, no clock continuation): the form to run under ncu")
     ap.add_argument("--config", type=int, default=2, choices=[2, 3, 5],
                     help="2 = the headline (default); 3 / 5 = the zoom-in engines of BASELINE.json configs[2] / configs[4]")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="headline config: write the last timed step's predictions to DIR/pred_corrs.npy (float32)")
     args = ap.parse_args()
     if args.gpus > 1 and "WORLD_SIZE" not in os.environ:
         # `python bench.py --gpus N` without a launcher: become `torch.distributed.run` with N ranks on this node

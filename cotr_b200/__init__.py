@@ -1,4 +1,4 @@
-"""cotr_b200 - B200-native (sm_100a) implementation of the COTR correspondence-inference hot path.
+"""cotr_b200 - H100-native (sm_90a) implementation of the COTR correspondence-inference hot path.
 
 Layout (mirrors the reference's packages for this path only):
   csrc/       hand-written CUDA kernels + the C ABI (include/cotr_b200.h)

@@ -1,7 +1,7 @@
-"""Build libcotr_b200.so (sm_100a only) in-tree with nvcc.  `python -m cotr_b200.build [--force]`.
+"""Build libcotr_b200.so (sm_90a only) in-tree with nvcc.  `python -m cotr_b200.build [--force]`.
 
 The library is a plain C-ABI shared object (include/cotr_b200.h): no torch, no pybind.  It is built in-tree
-(cotr_b200/lib/) so that it travels to the GPU box with the repository snapshot.
+(cotr_b200/lib/) so that the package is importable straight from the repository tree.
 """
 import os
 import subprocess
@@ -13,7 +13,7 @@ CSRC = os.path.join(HERE, "csrc")
 LIB_DIR = os.path.join(HERE, "lib")
 LIB_PATH = os.path.join(LIB_DIR, "libcotr_b200.so")
 SOURCES = ["model.cu", "gemm_simt.cu", "gemm_tc.cu", "attention_simt.cu", "attention_tc.cu", "elementwise.cu", "preprocess.cu", "dense_post.cu", "engine_ops.cu", "peer_exchange.cu"]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "-Xptxas", "-v"]
 
 

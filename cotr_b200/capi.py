@@ -1,6 +1,6 @@
 """ctypes binding of the C ABI declared in include/cotr_b200.h.
 
-There is deliberately no CPU fallback: if the shared library is missing or no sm_100 GPU is visible the calls raise.
+There is deliberately no CPU fallback: if the shared library is missing or no sm_90 GPU is visible the calls raise.
 """
 import ctypes
 import os
@@ -86,7 +86,7 @@ def lib():
             try:
                 fn = getattr(handle, name)
             except AttributeError:
-                if os.environ.get("COTR_B200_ALLOW_OLD_LIB"):       # tools/ab_libs.py: A/B against a build of an older revision
+                if os.environ.get("COTR_B200_ALLOW_OLD_LIB"):       # A/B against a build of an older revision
                     continue
                 raise
             fn.restype = restype
@@ -138,7 +138,7 @@ class NativeModel:
 
     def __init__(self, state_dict, device_index):
         if not torch.cuda.is_available():
-            raise RuntimeError("cotr_b200 needs a CUDA device (sm_100a); there is no CPU fallback")
+            raise RuntimeError("cotr_b200 needs a CUDA device (sm_90a); there is no CPU fallback")
         names, arrays = [], []
         for k, v in state_dict.items():
             a = v.detach().to("cpu", torch.float32).contiguous().numpy() if isinstance(v, torch.Tensor) else np.ascontiguousarray(v, np.float32)
@@ -353,7 +353,7 @@ def rasterize_triangles(tris, H, W):
 def test_gemm(path, A, w_host, *, bias=None, addmat=None, add_period=1, residual=None, relu=False, ln=None,
               a_mode=0, conv=None, M=None, ldc=None, a_ln=False, res_ln=False, part_out=None):
     """Kernel-level hook: out = epilogue(A W^T).  A and optional epilogue operands are CUDA fp32 tensors.
-    a_ln / res_ln: `ln` = (gamma, beta) is a DEFERRED LayerNorm of the A rows / of the residual rows (tcgen05 path)."""
+    a_ln / res_ln: `ln` = (gamma, beta) is a DEFERRED LayerNorm of the A rows / of the residual rows (tensor-core path)."""
     N, K = w_host.shape
     d = TestGemmDesc()
     d.path = path

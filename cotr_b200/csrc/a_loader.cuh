@@ -1,5 +1,5 @@
 // Row/element addressing of the GEMM A operand (implicit im2col for the backbone convolutions).
-// Shared by the fp32 SIMT GEMM and the tcgen05 GEMM so both see exactly the same operand.
+// Shared by the fp32 SIMT GEMM and the wgmma GEMM so both see exactly the same operand.
 #pragma once
 #include "split16.cuh"
 

@@ -1,4 +1,4 @@
-// Shared declarations of the cotr_b200 CUDA library (sm_100a only).
+// Shared declarations of the cotr_b200 CUDA library (sm_90a only).
 #pragma once
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
@@ -29,15 +29,15 @@ void set_error(const char* fmt, ...);
 
 // ---------------------------------------------------------------------------------------------------------------
 // Programmatic dependent launch.  Every kernel of the forward is launched with the programmatic-stream-serialization
-// attribute: it may start (barrier init, TMEM allocation, weight prefetch by TMA) while its predecessor in the
+// attribute: it may start (barrier init, weight prefetch by TMA) while its predecessor in the
 // stream / graph is still draining, and calls pdl_wait() before it first touches memory the predecessor produces
 // (or still reads).  At batch 1 the forward is ~135 latency-bound launches, so hiding launch + prologue matters.
 // ---------------------------------------------------------------------------------------------------------------
 extern int g_use_pdl;
-extern long long* g_tc_timestamps;   // debug timeline buffer of the tcgen05 kernels (cotr_debug_set_timestamps), else null
+extern long long* g_tc_timestamps;   // debug timeline buffer of the tensor-core kernels (cotr_debug_set_timestamps), else null
 extern int g_tc_variant;
 extern int g_tc_trace_idx;
-// Trace mode (cotr_debug_set_variant bit 17 + a timestamp buffer): every tcgen05 launch gets its own block of
+// Trace mode (cotr_debug_set_variant bit 17 + a timestamp buffer): every tensor-core launch gets its own block of
 // 256 CTAs x 64 slots, so one forward (graph replay included) leaves a per-launch record; slots 61-63 hold %globaltimer.
 inline long long* next_trace_block() {
     if (!g_tc_timestamps) return nullptr;
@@ -173,6 +173,9 @@ inline cudaError_t launch_kernel_cluster(void (*kernel)(KArgs...), dim3 grid, di
     return cudaLaunchKernelEx(&cfg, kernel, KArgs(args)...);
 }
 
+// Streaming multiprocessors of an H100 SXM: grid-stride kernels launch at most 16 blocks per SM.
+constexpr int kNumSms = 132;
+
 constexpr int kDModel = 256;
 constexpr int kHeads = 8;
 constexpr int kHeadDim = 32;
@@ -184,7 +187,7 @@ constexpr int kDecLayers = 6;
 // Attention operand images (tensor-core path).  The keys and values of one (pair, slot, head) - slot = decoder layer, or 0
 // for the encoder's own layer - are stored in HBM exactly as the attention kernel wants them in shared memory, so that
 // staging them is two bulk-TMA copies issued by one thread (cp.async.bulk -> UBLKCP) instead of 8 192 16-byte cp.async:
-//   K image  [plane hi | lo][4 groups of 8 head dims][512 keys][16 B]           = 2 x 32 KB  (UMMA K-major canonical layout)
+//   K image  [plane hi | lo][4 groups of 8 head dims][512 keys][16 B]           = 2 x 32 KB  (wgmma K-major canonical layout)
 //   V image  [64 groups of 8 keys][hi: 32 head dims x 16 B | lo: 32 x 16 B | 16 B pad]  = 64 x 1040 B
 // written in that form by the epilogue of the projection GEMM (split16.cuh::store16).
 constexpr size_t kAttnKPlaneBytes = 4 * 512 * 16;                         // 32 KB
@@ -254,7 +257,7 @@ struct GemmParams {
     int relu;
     const float* ln_gamma;   // optional LayerNorm over the N = 256 columns of each row (after the residual)
     const float* ln_beta;
-    // Deferred LayerNorm (tcgen05 path, row-major A).  A LayerNorm output is never stored: the GEMM that produces the
+    // Deferred LayerNorm (tensor-core path, row-major A).  A LayerNorm output is never stored: the GEMM that produces the
     // PRE-norm rows x (N = 256) also leaves, per row and 16-column chunk, the chunk's (mean, M2) in `ln_part_out`
     // [M][16] float2 (from the fp32 values in its epilogue registers); every consumer merges the 16 pairs into the row's
     // (mean, rstd) in its own epilogue prologue and applies the norm on the fly:

@@ -213,7 +213,7 @@ __global__ void split16_to_f32_kernel(const CSplit16 in, float* __restrict__ out
 
 int grid_for(size_t total, int block) {
     const size_t blocks = (total + block - 1) / block;
-    return (int)(blocks < 148 * 16 ? (blocks ? blocks : 1) : 148 * 16);
+    return (int)(blocks < kNumSms * 16 ? (blocks ? blocks : 1) : kNumSms * 16);
 }
 
 }  // namespace

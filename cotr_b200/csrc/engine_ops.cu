@@ -62,7 +62,7 @@ int rasterize_triangles_launch(const float* tris, int n_tri, int H, int W, float
     COTR_CHECK(out != nullptr && H > 0 && W > 0 && n_tri >= 0 && (n_tri == 0 || tris != nullptr), "cotr_rasterize_triangles: bad arguments");
     COTR_CHECK_CUDA(cudaMemsetAsync(out, 0, (size_t)H * W * 2 * sizeof(float), s));
     if (n_tri == 0) return 0;
-    const int grid = n_tri < 148 * 8 ? n_tri : 148 * 8;
+    const int grid = n_tri < kNumSms * 8 ? n_tri : kNumSms * 8;
     rasterize_triangles_kernel<<<grid, 256, 0, s>>>(reinterpret_cast<const Vtx*>(tris), n_tri, H, W, reinterpret_cast<float2*>(out));
     COTR_CHECK_CUDA(cudaGetLastError());
     return 0;
@@ -242,7 +242,7 @@ int flow_tile_merge_launch(FlowMerger* f, const float* tile, int pitch, const do
         f->tmp_cap = need;
     }
     if (first) {
-        flow_init_kernel<<<148 * 4, 256, 0, s>>>(flow, conf, (size_t)ow * oh);
+        flow_init_kernel<<<kNumSms * 4, 256, 0, s>>>(flow, conf, (size_t)ow * oh);
         COTR_CHECK_CUDA(cudaGetLastError());
     }
     flow_resize_h_kernel<<<(kTileIn * pw + 255) / 256, 256, 0, s>>>(j, f->tmp);

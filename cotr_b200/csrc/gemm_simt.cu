@@ -1,5 +1,5 @@
 // fp32 SIMT GEMM on split16 activations with the same implicit-im2col A addressing and the same epilogue contract as
-// the tcgen05 GEMM.  Numerical cross-check path (cotr_set_gemm_path(m, 1): plain fp32 FMA arithmetic on the
+// the wgmma GEMM.  Numerical cross-check path (cotr_set_gemm_path(m, 1): plain fp32 FMA arithmetic on the
 // reconstructed hi + lo values) and the producer of the constant position-bias matrices at model creation.
 #include "a_loader.cuh"
 

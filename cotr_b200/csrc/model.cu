@@ -114,7 +114,7 @@ struct cotr_context {
 
 struct cotr_model {
     int device = 0;
-    int gemm_path = 0;          // 0 = tcgen05, 1 = fp32 SIMT
+    int gemm_path = 0;          // 0 = tensor cores (wgmma), 1 = fp32 SIMT
     int launches = 0;
     std::vector<void*> allocs;
     cotr::DevConv stem;
@@ -397,7 +397,7 @@ GemmParams gemm_base(int M, int N, int K, CSplit16 A, int lda, const float* W, c
     return p;
 }
 
-// One tcgen05 GEMM launch with its dataflow bookkeeping.  dep_mode: DEP_ALL / DEP_TILE (the A rows of a CTA's tile come
+// One tensor-core GEMM launch with its dataflow bookkeeping.  dep_mode: DEP_ALL / DEP_TILE (the A rows of a CTA's tile come
 // from the same 128-row tile of the previous launch, and nothing this launch overwrites is still read by other tiles).
 int launch_tc(const Run& r, GemmParams& p, int dep_mode = DEP_ALL) {
     // only the row-major operand kernels exist in a dataflow-capable form (gemm_tc.cu, DLN instantiations): convolutions
@@ -564,11 +564,10 @@ int ensure_sync_ctr(cotr_model* m) {
     return 0;
 }
 // bring-up switch: cotr_debug_set_variant bit 18 turns the dataflow dependencies off (hardware griddepcontrol.wait everywhere)
-// Schedule selection (profiles/r02_deferred_layernorm.md has the measurements behind it).
+// Schedule selection.
 // Deferred LayerNorm (no LayerNorm launches; consumers normalise on the fly) removes 12 launches from the encoder and
-// 12 from each decoder chunk but makes its consumer GEMMs a little longer: on B200 it loses 2.4% on the 512-token /
-// 1024-row chains of the headline shape and wins 3-5% once a section has thousands of rows, so each section picks it
-// by its row count.  cotr_debug_set_variant overrides: bit 19 = always deferred, bit 16 = never.  Bits 19 + 18 together
+// 12 from each decoder chunk but makes its consumer GEMMs a little longer: it pays off only once a section has
+// thousands of rows (the launches saved then outweigh the longer epilogues), so each section picks it by its row count.  cotr_debug_set_variant overrides: bit 19 = always deferred, bit 16 = never.  Bits 19 + 18 together
 // additionally swap griddepcontrol.wait for the counter-based dataflow dependencies of common.cuh - measured slower
 // everywhere, opt-in only.
 constexpr int kDeferredLnMinRows = 2048;
@@ -683,7 +682,7 @@ int encode_impl(cotr_model* m, const float* img, int B, cotr_context* ctx, cudaS
         LaunchSync y = plan_dep(r, DEP_ALL, n_img * 256 * 256);
         if (launch_stem_canvas(img, w.canvas, n_img, s, y)) return 1;
         const size_t blocks = ((size_t)n_img * 256 * 256 + 255) / 256;
-        plan_done(r, y, (int)(blocks < 148 * 16 ? blocks : 148 * 16), 0, n_img * 256 * 256);
+        plan_done(r, y, (int)(blocks < kNumSms * 16 ? blocks : kNumSms * 16), 0, n_img * 256 * 256);
     }
     if (run_conv(r, m->stem, n_img, cs(w.canvas), 256, 256, w.stem, true, none)) return 1;
     {
@@ -692,7 +691,7 @@ int encode_impl(cotr_model* m, const float* img, int B, cotr_context* ctx, cudaS
         if (launch_maxpool_3x3s2_nhwc(cs(w.stem), w.bx, n_img, 128, 128, 64, s, y)) return 1;
         const size_t total = (size_t)n_img * 64 * 64 * 8;
         const size_t blocks = (total + 255) / 256;
-        plan_done(r, y, (int)(blocks < 148 * 16 ? blocks : 148 * 16), 0, n_img * 64 * 64);
+        plan_done(r, y, (int)(blocks < kNumSms * 16 ? blocks : kNumSms * 16), 0, n_img * 64 * 64);
     }
 
     Split16 x = w.bx;
@@ -1169,7 +1168,7 @@ using namespace cotr;
 extern "C" {
 
 const char* cotr_last_error(void) { return g_error; }
-const char* cotr_version(void) { return "cotr_b200 0.2 (sm_100a)"; }
+const char* cotr_version(void) { return "cotr_b200 0.3 (sm_90a)"; }
 
 int cotr_create(int device, const cotr_tensor* tensors, int n_tensors, cotr_model** out) {
     COTR_CHECK(out != nullptr && tensors != nullptr && n_tensors > 0, "cotr_create: bad arguments");
@@ -1180,7 +1179,7 @@ int cotr_create(int device, const cotr_tensor* tensors, int n_tensors, cotr_mode
     COTR_CHECK_CUDA(cudaSetDevice(device));
     cudaDeviceProp prop;
     COTR_CHECK_CUDA(cudaGetDeviceProperties(&prop, device));
-    COTR_CHECK(prop.major == 10, "cotr_create: this library is built for sm_100a only; device %d is sm_%d%d", device, prop.major, prop.minor);
+    COTR_CHECK(prop.major == 9 && prop.minor == 0, "cotr_create: this library is built for sm_90a only; device %d is sm_%d%d", device, prop.major, prop.minor);
     TensorMap tm;
     for (int i = 0; i < n_tensors; ++i) {
         COTR_CHECK(tensors[i].name != nullptr, "cotr_create: tensor %d has no name", i);
@@ -1512,7 +1511,7 @@ int64_t cotr_debug_read(cotr_model* m, const char* name, float* out_host, int64_
 }
 
 int cotr_set_gemm_path(cotr_model* m, int path) {
-    COTR_CHECK(m && (path == 0 || path == 1), "cotr_set_gemm_path: path must be 0 (tcgen05) or 1 (fp32 SIMT)");
+    COTR_CHECK(m && (path == 0 || path == 1), "cotr_set_gemm_path: path must be 0 (tensor cores) or 1 (fp32 SIMT)");
     if (m->gemm_path != path) {          // captured graphs embed the kernels of the old path
         cudaSetDevice(m->device);
         cudaDeviceSynchronize();

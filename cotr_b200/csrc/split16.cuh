@@ -1,4 +1,4 @@
-// fp32 <-> split16 (fp16 hi + fp16 lo) conversions and the GEMM epilogue store shared by the SIMT and tcgen05 kernels.
+// fp32 <-> split16 (fp16 hi + fp16 lo) conversions and the GEMM epilogue store shared by the SIMT and wgmma kernels.
 #pragma once
 #include "common.cuh"
 
@@ -34,8 +34,7 @@ __device__ __forceinline__ float join_f16(__half hi, __half lo) { return __half2
 // Activations are read with ld.global.cg, never through the non-coherent path (__ldg / ld.global.nc): under
 // programmatic dependent launch a kernel is resident while its predecessor still writes these buffers, so they are not
 // read-only for the kernel's lifetime, which .nc requires - measured: an SM's L1 kept row statistics of the PREVIOUS
-// forward across the launches in between and a .nc load after griddepcontrol.wait returned them
-// (profiles/r02_deferred_layernorm.md).  Constants (weights, biases, gamma / beta, tables) keep __ldg.
+// forward across the launches in between and a .nc load after griddepcontrol.wait returned them.  Constants (weights, biases, gamma / beta, tables) keep __ldg.
 __device__ __forceinline__ void load8_split(const CSplit16& t, size_t off, float (&v)[8]) {
     const uint4 h = __ldcg(reinterpret_cast<const uint4*>(t.hi + off));
     const uint4 l = __ldcg(reinterpret_cast<const uint4*>(t.lo + off));

@@ -1,5 +1,6 @@
-// Thin inline-PTX layer for sm_100a: mbarrier, cp.async, bulk TMA (cp.async.bulk), tcgen05 MMA / TMEM.
-// No CUTLASS dependency; descriptor bit layouts follow the PTX ISA "tcgen05 matrix / instruction descriptor".
+// Thin inline-PTX layer for sm_90a: mbarrier, cp.async, bulk TMA (cp.async.bulk), thread-block clusters and wgmma
+// (warpgroup MMA, accumulators in registers).  No CUTLASS dependency; descriptor bit layouts follow the PTX ISA
+// "wgmma matrix descriptor".
 #pragma once
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
@@ -41,16 +42,15 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
     }
 }
 
-// generic-proxy writes (st.shared) -> visible to the async proxy (tcgen05.mma / TMA reads of shared memory)
+// generic-proxy writes (st.shared) -> visible to the async proxy (wgmma / TMA reads of shared memory)
 __device__ __forceinline__ void fence_proxy_async_smem() {
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 }
 
-// ---- 256-bit global load through L2 only (LDG.E.ENL2.256): 32-byte aligned address --------------------------------
-__device__ __forceinline__ void ld_cg_256(const void* p, uint4& a, uint4& b) {
-    asm volatile("ld.global.cg.v8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-                 : "=r"(a.x), "=r"(a.y), "=r"(a.z), "=r"(a.w), "=r"(b.x), "=r"(b.y), "=r"(b.z), "=r"(b.w)
-                 : "l"(p));
+// ---- 32 bytes (one sector) through L2 only: two 16-byte ld.global.cg ----------------------------------------------
+__device__ __forceinline__ void ld_cg_32b(const void* p, uint4& a, uint4& b) {
+    a = __ldcg(reinterpret_cast<const uint4*>(p));
+    b = __ldcg(reinterpret_cast<const uint4*>(p) + 1);
 }
 
 // ---- cp.async (LDGSTS): 16 bytes global -> shared, zero-filled when src_bytes == 0 --------------------------------
@@ -100,99 +100,70 @@ __device__ __forceinline__ void tma_bulk_g2s(void* smem_dst, const void* gmem_sr
                  : "memory");
 }
 
-// ---- TMEM allocation ---------------------------------------------------------------------------
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_result, uint32_t ncols) {   // whole warp, ncols pow2 >= 32
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_result)), "r"(ncols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {          // same warp that allocated
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tcgen05_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tcgen05_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// ---- descriptors -------------------------------------------------------------------------------
-// Shared-memory matrix descriptor, K-major, no swizzle.  Canonical layout in 16-byte units
-// ((8, n), 2) : ((1, SBO), LBO): a core matrix is 8 rows x 16 bytes stored contiguously (128 B),
-// SBO = byte distance between 8-row groups, LBO = byte distance between the two 16-byte K halves of one MMA.
-// Low word: start address >> 4 (bits 0-13), LBO >> 4 (bits 16-29).  High word: SBO >> 4 (bits 0-13), version 1 (bit 14).
-__device__ __forceinline__ uint32_t desc_hi(uint32_t sbo_bytes) { return ((sbo_bytes >> 4) & 0x3FFFu) | (1u << 14); }
-__device__ __forceinline__ uint32_t desc_lo(uint32_t smem_addr, uint32_t lbo_bytes) {
-    return ((smem_addr & 0x3FFFFu) >> 4) | (((lbo_bytes >> 4) & 0x3FFFu) << 16);
-}
-__device__ __forceinline__ uint64_t make_desc(uint32_t lo, uint32_t hi) { return (uint64_t)lo | ((uint64_t)hi << 32); }
+// ---- wgmma ---------------------------------------------------------------------------------------------------------
+// Shared-memory matrix descriptor (sm_90): start address >> 4 (bits 0-13), leading byte offset >> 4 (bits 16-29),
+// stride byte offset >> 4 (bits 32-45), layout type (bits 62-63: 0 = no swizzle, 1 = 128-byte swizzle).
+// K-major, no swizzle: a core matrix is 8 rows x 16 bytes stored contiguously (128 B); SBO = byte distance between
+// 8-row groups, LBO = byte distance between the two 16-byte K halves of one k16 step.
 __device__ __forceinline__ uint64_t make_smem_desc(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
-    return make_desc(desc_lo(smem_addr, lbo_bytes), desc_hi(sbo_bytes));
+    const uint32_t lo = ((smem_addr & 0x3FFFFu) >> 4) | (((lbo_bytes >> 4) & 0x3FFFu) << 16);
+    const uint32_t hi = (sbo_bytes >> 4) & 0x3FFFu;
+    return (uint64_t)lo | ((uint64_t)hi << 32);
 }
-
 // SWIZZLE_128B K-major operand tile: rows of 128 bytes (64 halves = one K chunk), 8-row groups 1024 bytes apart, the
-// 16-byte chunk c of row r stored at chunk position c ^ (r % 8) (tile base 1024-byte aligned).  LBO is not used by the
-// hardware in this mode (encoded as 1 like CUTLASS), SBO = 1024, layout_type = 2.  A K step of 16 halves advances the
-// start address by 32 bytes inside the swizzle atom.
-__device__ __forceinline__ uint32_t desc_hi_sw128() { return (1024u >> 4) | (1u << 14) | (2u << 29); }
-__device__ __forceinline__ uint32_t desc_lo_sw128(uint32_t smem_addr) { return ((smem_addr & 0x3FFFFu) >> 4) | (1u << 16); }
-
-// Instruction descriptor for kind::f16: FP16 x FP16 -> FP32 (a_format = b_format = 0), both operands K-major, dense.
-__host__ __device__ constexpr uint32_t make_idesc_f16_f32(int M, int N) {
-    return (1u << 4)                      // c_format = F32
-           | ((uint32_t)(N >> 3) << 17)   // n_dim
-           | ((uint32_t)(M >> 4) << 24);  // m_dim
+// 16-byte chunk c of row r stored at chunk position c ^ (r % 8) (tile base 1024-byte aligned).  LBO is not used in
+// this mode (encoded as 1), SBO = 1024.  A k16 step advances the start address by 32 bytes inside the swizzle atom;
+// a sub-tile that starts a multiple of 1024 bytes further keeps the swizzle phase.
+__device__ __forceinline__ uint64_t make_desc_sw128(uint32_t smem_addr) {
+    const uint32_t lo = ((smem_addr & 0x3FFFFu) >> 4) | (1u << 16);
+    const uint32_t hi = (1024u >> 4) | (1u << 30);
+    return (uint64_t)lo | ((uint64_t)hi << 32);
 }
 
-// D[tmem] (+)= A[smem] * B[smem]^T, issued by ONE thread on behalf of the CTA.
-__device__ __forceinline__ void umma_f16_ss(uint32_t tmem_d, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, bool accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(tmem_d), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"((uint32_t)accumulate)
-        : "memory");
-}
-
-// All previously issued MMAs of this thread arrive on `bar` when complete (implies fence::before_thread_sync).
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-
-// ---- TMEM <-> registers: 32 lanes x 16 consecutive fp32 columns per warp --------------------------
-// tmem_ld16_issue starts the load; the registers may only be consumed after tmem_ld16_fence on the SAME array (the
-// fence is a tcgen05.wait::ld that carries the registers as in/out operands, so the compiler cannot move uses above it).
-__device__ __forceinline__ void tmem_ld16_issue(uint32_t taddr, uint32_t (&r)[16]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-          "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-        : "r"(taddr));
-}
-__device__ __forceinline__ void tmem_ld16_fence(uint32_t (&r)[16]) {
-    asm volatile("tcgen05.wait::ld.sync.aligned;"
-                 : "+r"(r[0]), "+r"(r[1]), "+r"(r[2]), "+r"(r[3]), "+r"(r[4]), "+r"(r[5]), "+r"(r[6]), "+r"(r[7]),
-                   "+r"(r[8]), "+r"(r[9]), "+r"(r[10]), "+r"(r[11]), "+r"(r[12]), "+r"(r[13]), "+r"(r[14]), "+r"(r[15])
-                 :
-                 : "memory");
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, float* v) {
-    uint32_t r[16];
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];\n\t"
-        "tcgen05.wait::ld.sync.aligned;"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-          "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-        : "r"(taddr)
-        : "memory");
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// Keeps the compiler from moving accesses to accumulator registers across wgmma issue / wait.
+template <int R>
+__device__ __forceinline__ void fence_regs(float (&d)[R]) {
 #pragma unroll
-    for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]);
+    for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
-__device__ __forceinline__ void tmem_st16(uint32_t taddr, const float* v) {
+
+// D[64 x N] (fp32, registers of the warpgroup) += A[64 x 16] * B[N x 16]^T, fp16 operands, both K-major in shared
+// memory (ss) or A from registers in the accumulator-fragment layout (rs).  Issued by all 128 threads of a warpgroup;
+// asynchronous until wgmma_commit + wgmma_wait.
+__device__ __forceinline__ void wgmma_ss_n16(float (&d)[8], uint64_t a_desc, uint64_t b_desc) {
     asm volatile(
-        "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16};"
-        ::"r"(taddr), "r"(__float_as_uint(v[0])), "r"(__float_as_uint(v[1])), "r"(__float_as_uint(v[2])), "r"(__float_as_uint(v[3])),
-          "r"(__float_as_uint(v[4])), "r"(__float_as_uint(v[5])), "r"(__float_as_uint(v[6])), "r"(__float_as_uint(v[7])),
-          "r"(__float_as_uint(v[8])), "r"(__float_as_uint(v[9])), "r"(__float_as_uint(v[10])), "r"(__float_as_uint(v[11])),
-          "r"(__float_as_uint(v[12])), "r"(__float_as_uint(v[13])), "r"(__float_as_uint(v[14])), "r"(__float_as_uint(v[15]))
-        : "memory");
+        "wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7}, %8, %9, 1, 1, 1, 0, 0;"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+        : "l"(a_desc), "l"(b_desc));
 }
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_ss_n32(float (&d)[16], uint64_t a_desc, uint64_t b_desc) {
+    asm volatile(
+        "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, %16, %17, 1, 1, 1, 0, 0;"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+        : "l"(a_desc), "l"(b_desc));
+}
+__device__ __forceinline__ void wgmma_ss_n64(float (&d)[32], uint64_t a_desc, uint64_t b_desc) {
+    asm volatile(
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, %32, %33, 1, 1, 1, 0, 0;"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "l"(a_desc), "l"(b_desc));
+}
+__device__ __forceinline__ void wgmma_ss_n128(float (&d)[64], uint64_t a_desc, uint64_t b_desc) {
+    asm volatile(
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, %64, %65, 1, 1, 1, 0, 0;"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "l"(a_desc), "l"(b_desc));
+}
+__device__ __forceinline__ void wgmma_rs_n32(float (&d)[16], const uint32_t (&a)[4], uint64_t b_desc) {
+    asm volatile(
+        "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, {%16,%17,%18,%19}, %20, 1, 1, 1, 0;"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b_desc));
+}
 
 }  // namespace tc
 }  // namespace cotr

@@ -1,4 +1,4 @@
-"""The COTR network as an nn.Module shell around the native sm_100a implementation.
+"""The COTR network as an nn.Module shell around the native sm_90a implementation.
 
 Reference contract (COTR/models/cotr_model.py:17-51):
   * `build(args)` -> module with attributes transformer (.d_model), corr_embed, query_proj, input_proj, backbone;
@@ -196,7 +196,7 @@ class COTR(nn.Module):
         if self._native is None:
             dev = next(self.parameters()).device
             if dev.type != "cuda":
-                raise RuntimeError("cotr_b200.COTR runs only on a CUDA device (sm_100a): call model.cuda() first; "
+                raise RuntimeError("cotr_b200.COTR runs only on a CUDA device (sm_90a): call model.cuda() first; "
                                    "there is no CPU fallback")
             idx = dev.index if dev.index is not None else torch.cuda.current_device()
             self._native = capi.NativeModel(self.state_dict(), idx)

@@ -1,5 +1,5 @@
 /*
- * cotr_b200 - C ABI of the B200-native COTR correspondence-inference hot path.
+ * cotr_b200 - C ABI of the H100-native COTR correspondence-inference hot path.
  *
  * This is the drop-in boundary: plain pointers and sizes, no torch types.  The
  * reference (ubc-vision/COTR) is pure Python, so "what its FFI would bind" is
@@ -171,7 +171,7 @@ int cotr_last_launch_count(const cotr_model* m);
 /* Per-launch profiler.  Between cotr_profile_begin and cotr_profile_end every kernel the library launches is bracketed
  * by two CUDA events recorded on the launching stream.  cotr_profile_end synchronises the device, fills `out` with
  * one record per launch in launch order and returns -(count + 1) on success (so 0 records -> -1), > 0 on failure.
- * kernel ids: 0 gemm_tc (tcgen05), 1 gemm_simt, 2 attention_tc, 3 attention_simt, 4 layernorm, 5 maxpool,
+ * kernel ids: 0 gemm_tc (wgmma), 1 gemm_simt, 2 attention_tc, 3 attention_simt, 4 layernorm, 5 maxpool,
  * 6 query_encode, 7 stem_canvas.  For GEMMs M,N,K are the problem size; for attention M = query rows, N = 512, K = 256. */
 typedef struct cotr_launch_record {
     int32_t kernel;
@@ -187,13 +187,13 @@ int cotr_profile_end(cotr_model* m, cotr_launch_record* out, int max_records);
  * Returns the element count copied, or -1. */
 int64_t cotr_debug_read(cotr_model* m, const char* name, float* out_host, int64_t max_elems);
 
-/* Select the matrix-multiply path: 0 = tcgen05 tensor-core kernels (default), 1 = fp32 SIMT kernels
+/* Select the matrix-multiply path: 0 = wgmma tensor-core kernels (default), 1 = fp32 SIMT kernels
  * (debug / numerical cross-check only). */
 int cotr_set_gemm_path(cotr_model* m, int path);
 
 /* ---- kernel-level test hooks (used by tests/ only) ------------------------------------------------------ */
 typedef struct cotr_test_gemm_desc {
-    int32_t path;                 /* 0 = tcgen05, 1 = fp32 SIMT                                               */
+    int32_t path;                 /* 0 = wgmma, 1 = fp32 SIMT                                                 */
     int32_t M, N, K;
     int32_t a_mode;               /* 0 row-major [M,K]; 1 implicit im2col over NHWC; 2 7x7/2 stem (A_dev = the fp32 (B,3,256,512) canvas, w_host [N][7][7][3]); 3 token gather */
     int32_t lda;
@@ -201,7 +201,7 @@ typedef struct cotr_test_gemm_desc {
     int32_t relu;
     int32_t add_period, ld_add, ldr, ldc;
     int32_t a_ln;                 /* 1: A holds PRE-LayerNorm rows (K = 256); ln_gamma / ln_beta are the norm of A,
-                                     applied on the fly (deferred LayerNorm, tcgen05 path only) instead of an output norm */
+                                     applied on the fly (deferred LayerNorm, wgmma path only)   instead of an output norm */
     int32_t res_ln;               /* 1: the residual (ldr = N = 256) is a deferred LayerNorm too, same gamma / beta   */
     int32_t emit_part;            /* 1: also write the [M][16] (mean, M2) partial row statistics of the output (N = 256) */
     int32_t reserved;
@@ -217,18 +217,18 @@ int cotr_test_gemm(const cotr_test_gemm_desc* d, const float* A_dev, const float
 int cotr_test_attention(int path, const float* q_dev, const float* k_dev, const float* v_dev, float* out_dev,
                         int nq, int npairs);
 /* bring-up / A-B switches (0 = production): bit 8 (256) disables programmatic dependent launch, bit 9 (512) disables
- * split-K, bits 10-11 / 12-13 move the CTA-count thresholds of the 64- / 128-wide GEMM tiles, bits 14-15 lower the
+ * split-K, bits 10-11 move the CTA-count threshold of the 64-wide GEMM tile, bits 14-15 lower the
  * minimum K of split-K (16 >> n chunks of 64), bit 17 selects trace mode for cotr_debug_set_timestamps, bits 20-22 stop
  * the encoder after n layers.  Schedule: by default a transformer section with >= 2048 rows runs the deferred-LayerNorm
  * schedule (no LayerNorm launches), smaller ones the explicit one; bit 19 forces deferred everywhere, bit 16 never;
- * bits 19 + 18 add the counter-based dataflow dependencies (experimental, slower - profiles/r02_deferred_layernorm.md).
+ * bits 19 + 18 add the counter-based dataflow dependencies (experimental).
  * Process-wide; graphs captured under another value are NOT dropped (call cotr_set_gemm_path twice to drop them). */
 void cotr_debug_set_variant(int variant);
-/* debug timeline of the tcgen05 kernels: DEVICE buffer of 64 int64 per CTA receiving clock64() deltas of the pipeline
+/* debug timeline of the tensor-core kernels: DEVICE buffer of 64 int64 per CTA receiving clock64() deltas of the pipeline
  * events of every following GEMM / attention launch (NULL switches it off; graph replay is off while it is set).
- * Slot layout: tools/bringup.py::gemm_timeline / attn_timeline.  Trace mode (variant bit 17): the buffer holds
+ * Slot layout: the COTR_TS marks in gemm_tc.cu / attention_tc.cu.  Trace mode (variant bit 17): the buffer holds
  * 256 x 64 slots PER LAUNCH (launch counter reset by this call), slot 62 receives %globaltimer at CTA exit, and graph
- * replay stays on - tools/bringup.py::forward_trace reconstructs a per-launch schedule of one forward from it. */
+ * replay stays on, so a per-launch schedule of one forward can be reconstructed from it. */
 void cotr_debug_set_timestamps(void* dev_buffer);
 
 const char* cotr_last_error(void);

@@ -1,4 +1,4 @@
-"""GPU: the zoom-in engines (cotr_b200.inference) driving the native sm_100a model, against the same engines driving
+"""GPU: the zoom-in engines (cotr_b200.inference) driving the native sm_90a model, against the same engines driving
 the CPU oracle.  The loop is discontinuous in the network output (integer crop corners, accept / reject thresholds),
 so the comparison is reported in pixels on forced queries (SURVEY.md section 7 "what engine-level parity can mean")."""
 import numpy as np

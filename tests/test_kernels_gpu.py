@@ -7,8 +7,8 @@ import torch.nn.functional as F
 pytestmark = pytest.mark.gpu
 
 TC, SIMT = 0, 1
-# relative (Frobenius) error bounds: fp32 SIMT accumulates in fp32; the tcgen05 path uses the fp16 hi/lo split
-# (3 products, fp32 accumulate in TMEM), which is fp32-class (gemm_tc.cu header)
+# relative (Frobenius) error bounds: fp32 SIMT accumulates in fp32; the wgmma path uses the fp16 hi/lo split
+# (3 products, fp32 accumulate in registers), which is fp32-class (gemm_tc.cu header)
 REL = {SIMT: 2e-6, TC: 2.5e-6}
 
 

@@ -188,7 +188,7 @@ def test_experimental_schedules_match_the_reference(golden_dir, built_lib, varia
     """The schedules cotr_debug_set_variant can force (bit 19: LayerNorms applied on the fly by their consumers from
     partial row statistics, everywhere; bits 19 + 18: launch-to-launch dependencies through counters in global memory
     instead of griddepcontrol.wait; bit 16: explicit LayerNorm launches everywhere - by default each section picks by
-    its row count, profiles/r02_deferred_layernorm.md) all stay correct: same goldens, same tolerance, eager and
+    its row count) all stay correct: same goldens, same tolerance, eager and
     graph-replayed, also for a batch whose query count is not a tile multiple."""
     from cotr_b200 import capi
     capi.lib().cotr_debug_set_variant(variant)

@@ -157,7 +157,7 @@ def run_config(config, rank, local_rank, world, steps=2, cpu_rate=None):
         return
     line = {"metric": metric, "value": value, "unit": "query-points/s", "n_gpus": world, "steps": steps,
             "ms_per_step": 1e3 * n_points / value, "higher_is_better": True, "scaling": "strong",
-            "dtype": "f32 (fp16 hi/lo split operands, fp32 accumulate on tcgen05)", "data": "synthetic",
+            "dtype": "f32 (fp16 hi/lo split operands, fp32 accumulate on wgmma)", "data": "synthetic",
             "config": {"workload": workload, "zoom_ins": [float(z) for z in ZOOMS], "batch_size": 32,
                        "parallelism": f"{world} rank(s), SPMD scheduler, contexts split contiguously per model call"},
             "engines": runs, "timing": "wall clock around the whole engine run (host scheduler included), max over ranks, median of the runs"}
