@@ -68,7 +68,6 @@ _PROTOTYPES = {
     "cotr_test_gemm": (ctypes.c_int, [ctypes.POINTER(TestGemmDesc)] + [ctypes.c_void_p] * 9),
     "cotr_test_attention": (ctypes.c_int, [ctypes.c_int] + [ctypes.c_void_p] * 4 + [ctypes.c_int, ctypes.c_int]),
     "cotr_debug_set_variant": (None, [ctypes.c_int]),
-    "cotr_debug_set_timestamps": (None, [ctypes.c_void_p]),
     "cotr_last_error": (ctypes.c_char_p, []),
     "cotr_version": (ctypes.c_char_p, []),
 }

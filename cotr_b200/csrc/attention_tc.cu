@@ -50,45 +50,34 @@ __device__ __forceinline__ float fast_exp2(float x) {
     return y;
 }
 
-__global__ void __launch_bounds__(kThreads, 1) attention_tc_kernel(const AttnParams p, long long* __restrict__ ts) {
-    // debug timeline (ts != null, cotr_debug_set_timestamps): 64 clock64() stamps per CTA (COTR_TS slots below)
-    long long* my_ts = ts ? ts + (size_t)((blockIdx.z * gridDim.y + blockIdx.y) * gridDim.x + blockIdx.x) * 64 : nullptr;
-    const long long t_start = ts ? clock64() : 0;
-#define COTR_TS(slot) do { if (my_ts) my_ts[(slot)] = clock64() - t_start; } while (0)
+// Capped at the 168 registers of the GEMM's budget: left free, the scheduler overlaps consecutive key chunks and takes
+// more (no gain in occupancy: shared memory already limits the SM to one CTA).
+__global__ void __maxnreg__(168) attention_tc_kernel(const AttnParams p) {
     extern __shared__ __align__(128) uint8_t smem[];
     uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kOffBar);
     uint64_t* qk_full = bars + 0;
     uint64_t* v_full = bars + 1;
-    uint64_t* dep_ready = bars + 2;  // dataflow mode (common.cuh LaunchSync): the polling thread has seen the producer's counters
-    uint64_t* k_img_full = bars + 3; // operand images: the bulk copy of K (hi + lo planes) has landed
+    uint64_t* k_img_full = bars + 2; // operand images: the bulk copy of K (hi + lo planes) has landed
     const bool img = p.kv_img != nullptr;       // keys / values arrive as operand images by bulk TMA (tensor-core schedule)
-    const bool dflow = p.sync.dep_mode != DEP_PDL;
 
     const int t = threadIdx.x;
     const int warp = t >> 5, lane = t & 31;
     const int head = blockIdx.y;
     const int pair_local = blockIdx.z;
     const int row0 = blockIdx.x * kTile;
-    const int sync_tile = (pair_local * p.nq + row0) / kTile;      // this CTA's 128-row tile of the launch's row space (nq % 128 == 0 in tile modes)
 
     if (t == 0) {
         mbar_init(qk_full, kThreads);
         mbar_init(v_full, img ? 1 : kThreads);
-        mbar_init(dep_ready, 1);
         mbar_init(k_img_full, 1);
         mbar_fence_init();
     }
     __syncthreads();
     const uint32_t sbase = smem_u32(smem);
-    if (t == 0) COTR_TS(1);
 
     const size_t kv_row0 = (size_t)(p.pair0 + pair_local) * kTokens;
-    if (t == 0) {
-        pdl_launch_dependents();                     // the next kernel may start its prologue on idle SMs
-        if (dflow) { dep_wait_thread(p.sync, sync_tile); mbar_arrive(dep_ready); }
-    }
-    if (dflow) mbar_wait(dep_ready, 0); else pdl_wait();      // prologue above overlaps the previous kernel
-    if (t == 0) COTR_TS(2);
+    if (t == 0) pdl_launch_dependents();             // the next kernel may start its prologue on idle SMs
+    pdl_wait();                                      // prologue above overlaps the previous kernel
 
     if (img && t == 0) {
         // keys and values of this (pair, head): two bulk-TMA copies (UBLKCP) of the operand images straight into the
@@ -144,7 +133,6 @@ __global__ void __launch_bounds__(kThreads, 1) attention_tc_kernel(const AttnPar
         }
         cp_async_mbar_arrive_noinc(v_full);
     }
-    if (t == 0) COTR_TS(3);
 
     // ---- online softmax over 64-key chunks ------------------------------------------------------------------------
     // Fragment of an m64nN accumulator: register 4 j + {0,1} = row (warp % 4) * 16 + lane / 4 ("row a"), columns
@@ -155,7 +143,6 @@ __global__ void __launch_bounds__(kThreads, 1) attention_tc_kernel(const AttnPar
     if (img) mbar_wait(k_img_full, 0);
     mbar_wait(v_full, 0);
     fence_proxy_async_smem();                            // cp.async (generic proxy) data -> wgmma (async proxy)
-    if (t == 0) COTR_TS(4);
     const float kLog2e = 1.4426950408889634f;
     float mx_a = -INFINITY, mx_b = -INFINITY, sum_a = 0.f, sum_b = 0.f;
     float om[2][16], oc[16];
@@ -232,7 +219,6 @@ __global__ void __launch_bounds__(kThreads, 1) attention_tc_kernel(const AttnPar
         wgmma_commit();
         wgmma_wait<0>();
         fence_regs(om[0]); fence_regs(om[1]); fence_regs(oc);
-        if (t == 0) COTR_TS(6 + c);
     }
     }
 #pragma unroll
@@ -263,13 +249,6 @@ __global__ void __launch_bounds__(kThreads, 1) attention_tc_kernel(const AttnPar
             }
         }
     }
-    if (t == 0) COTR_TS(15);
-
-    __syncthreads();
-    if (t == 0) dep_signal_thread(p.sync, sync_tile);
-    if (t == 0) COTR_TS(60);
-    if (my_ts && t == 0) my_ts[62] = global_ns();
-#undef COTR_TS
 }
 
 }  // namespace
@@ -285,7 +264,7 @@ int launch_attention_tc(const AttnParams& p, cudaStream_t s) {
     COTR_CHECK((p.ldq & 7) == 0 && (p.ldk & 7) == 0 && (p.ldo & 7) == 0 && (p.vt_pair_stride & 7) == 0,
                "attention_tc: leading dimensions must be multiples of 8 elements");
     dim3 grid((p.nq + kTile - 1) / kTile, kHeads, p.npairs);
-    COTR_CHECK_CUDA(launch_kernel(attention_tc_kernel, grid, dim3(kThreads), kSmemBytes, s, p, next_trace_block()));
+    COTR_CHECK_CUDA(launch_kernel(attention_tc_kernel, grid, dim3(kThreads), kSmemBytes, s, p));
     return 0;
 }
 

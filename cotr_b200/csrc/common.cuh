@@ -34,89 +34,10 @@ void set_error(const char* fmt, ...);
 // (or still reads).  At batch 1 the forward is ~135 latency-bound launches, so hiding launch + prologue matters.
 // ---------------------------------------------------------------------------------------------------------------
 extern int g_use_pdl;
-extern long long* g_tc_timestamps;   // debug timeline buffer of the tensor-core kernels (cotr_debug_set_timestamps), else null
 extern int g_tc_variant;
-extern int g_tc_trace_idx;
-// Trace mode (cotr_debug_set_variant bit 17 + a timestamp buffer): every tensor-core launch gets its own block of
-// 256 CTAs x 64 slots, so one forward (graph replay included) leaves a per-launch record; slots 61-63 hold %globaltimer.
-inline long long* next_trace_block() {
-    if (!g_tc_timestamps) return nullptr;
-    if (!(g_tc_variant & (1 << 17))) return g_tc_timestamps;
-    return g_tc_timestamps + (size_t)(g_tc_trace_idx++) * 64 * 256;
-}
 #ifdef __CUDACC__
-__device__ __forceinline__ long long global_ns() {
-    long long t;
-    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-    return t;
-}
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 __device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
-#endif
-
-// ---------------------------------------------------------------------------------------------------------------
-// Launch-to-launch dependencies through counters in global memory ("dataflow" mode of the forward chain).
-// griddepcontrol.wait releases a dependent grid only when the WHOLE producer grid has retired and its memory is flushed
-// (measured 0.7-1.3 us after the producer's last CTA, plus the start skew of the producer's CTAs).  In dataflow mode
-// every CTA announces its finished stores on a counter block of its launch (block[0]: all CTAs, block[1 + t]: the CTAs
-// that wrote rows of the 128-row tile t) with a gpu-scope release, and a consumer CTA waits - one polling thread, then
-// an mbarrier / __syncthreads for the rest of the CTA - only for what it reads:
-//   DEP_ALL    every CTA of the producer                                   block[0]      >= dep_target
-//   DEP_TILE   the producer CTAs of this CTA's own 128-row tile            block[1 + t]  >= dep_target
-//   DEP_SPAN   the producer CTAs of dep_span consecutive tiles starting at (t / dep_span) * dep_span (attention: keys
-//              and values of the whole image pair)
-// The launches keep the programmatic-stream-serialization attribute (a consumer becomes resident early) but do not
-// execute griddepcontrol.wait.  No deadlock: a grid is only launched once every CTA of its producer is resident or done.
-// Counters are zeroed by one memset at the head of the forward.  dep_mode == DEP_PDL keeps the hardware wait.
-// ---------------------------------------------------------------------------------------------------------------
-enum DepMode : int { DEP_PDL = 0, DEP_ALL = 1, DEP_TILE = 2, DEP_SPAN = 3 };
-constexpr int kSyncBlockInts = 256;        // ints per launch: [0] total, [1 .. 255] per 128-row tile
-struct LaunchSync {
-    const int* dep;       // counter block of the producer launch
-    int dep_mode;
-    int dep_target;       // signals expected on each counter that is waited for
-    int dep_span;         // DEP_SPAN: tiles per group
-    int* sig;             // counter block of this launch (null: no announcement)
-    int sig_tiles;        // per-tile counters in use (0: only the total)
-};
-
-#ifdef __CUDACC__
-__device__ __forceinline__ int ld_acquire_gpu(const int* p) {
-    int v;
-    asm volatile("ld.acquire.gpu.global.s32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
-    return v;
-}
-// One thread: spin until *p >= target.  A counter that never arrives would hang the GPU, so the spin is bounded
-// (~2 s) and traps: the failure is loud and the device survives.
-__device__ __forceinline__ void dep_spin(const int* p, int target) {
-    long long t0 = 0;
-    unsigned spins = 0;
-    while (ld_acquire_gpu(p) < target) {
-        if ((++spins & 0xFFFu) == 0) {
-            const long long now = clock64();
-            if (t0 == 0) t0 = now;
-            else if (now - t0 > 4000000000ll) __trap();
-        }
-    }
-}
-// tile = this CTA's 128-row tile in the producer's row space
-__device__ __forceinline__ void dep_wait_thread(const LaunchSync& y, int tile) {
-    if (y.dep_mode == DEP_ALL) {
-        dep_spin(y.dep, y.dep_target);
-    } else if (y.dep_mode == DEP_TILE) {
-        dep_spin(y.dep + 1 + tile, y.dep_target);
-    } else if (y.dep_mode == DEP_SPAN) {
-        const int t0 = (tile / y.dep_span) * y.dep_span;
-        for (int t = 0; t < y.dep_span; ++t) dep_spin(y.dep + 1 + t0 + t, y.dep_target);
-    }
-}
-// One thread, after a CTA-wide barrier that follows the CTA's last global store.
-__device__ __forceinline__ void dep_signal_thread(const LaunchSync& y, int tile) {
-    if (y.sig == nullptr) return;
-    __threadfence();
-    atomicAdd(y.sig, 1);
-    if (y.sig_tiles > 0 && tile < y.sig_tiles) atomicAdd(y.sig + 1 + tile, 1);
-}
 #endif
 
 // Function attributes (opt-in dynamic shared memory) are per device, and one process may hold one handle per device:
@@ -270,7 +191,6 @@ struct GemmParams {
     const float* res_ln_gamma;
     const float* res_ln_beta;
     float2* ln_part_out;           // [M][16]; null = no statistics wanted
-    LaunchSync sync;         // dataflow dependencies (all zero: hardware griddepcontrol.wait)
     // outputs
     float* out_f32;          // when non-null: plain fp32 row-major output (the final prediction, N = 2)
     Split16 out;             // otherwise split16, row-major with leading dimension ldc ...
@@ -303,26 +223,23 @@ struct AttnParams {
     int nq;                      // query rows per pair in this launch
     int npairs;
     int pair0;
-    LaunchSync sync;             // dataflow dependencies (all zero: hardware griddepcontrol.wait)
 };
 
 int launch_gemm_simt(const GemmParams& p, cudaStream_t s);
 int launch_gemm_simt_raw(const GemmParams& p, float* raw_out_f32, cudaStream_t s);   // result as plain fp32 [M,N]
 int launch_layernorm_f32(const float* x, const float* gamma, const float* beta, Split16 out, int rows, cudaStream_t s);
-struct GemmLaunchInfo { int row_tiles, col_tiles, ksplit; };      // the grid launch_gemm_tc chose (dataflow bookkeeping)
-int launch_gemm_tc(const GemmParams& p, cudaStream_t s, GemmLaunchInfo* info = nullptr);
+int launch_gemm_tc(const GemmParams& p, cudaStream_t s);
 int launch_attention_simt(const AttnParams& p, cudaStream_t s);
 int launch_attention_tc(const AttnParams& p, cudaStream_t s);
-int launch_maxpool_3x3s2_nhwc(CSplit16 in, Split16 out, int N, int H, int W, int C, cudaStream_t s, LaunchSync sync = LaunchSync{});
+int launch_maxpool_3x3s2_nhwc(CSplit16 in, Split16 out, int N, int H, int W, int C, cudaStream_t s);
 int launch_layernorm(CSplit16 x, const float* gamma, const float* beta, Split16 out, int rows, cudaStream_t s);
 // out = LN2(LN1(x)): the last decoder layer's norm3 followed by decoder.norm (transformer.py:110-111) in one pass
 // part[row][c] = (mean, M2) of channels [16c, 16c+16) of a [rows][256] tensor (what GemmParams::ln_part_out holds)
 int launch_ln_partials(CSplit16 x, float2* part, int rows, cudaStream_t s);
-int launch_layernorm_twice(CSplit16 x, const float* g1, const float* b1, const float* g2, const float* b2, Split16 out, int rows, cudaStream_t s,
-                           LaunchSync sync = LaunchSync{});
-int launch_query_encode(const float* queries, Split16 qpos, int rows, cudaStream_t s, LaunchSync sync = LaunchSync{});
+int launch_layernorm_twice(CSplit16 x, const float* g1, const float* b1, const float* g2, const float* b2, Split16 out, int rows, cudaStream_t s);
+int launch_query_encode(const float* queries, Split16 qpos, int rows, cudaStream_t s);
 // fp32 (B,3,256,512) canvas -> the stem's bordered split16 NHWC4 operand (2B images of kStemCanvasElems halves per plane)
-int launch_stem_canvas(const float* img, Split16 canvas, int n_img, cudaStream_t s, LaunchSync sync = LaunchSync{});
+int launch_stem_canvas(const float* img, Split16 canvas, int n_img, cudaStream_t s);
 int launch_f32_to_split16(const float* in, Split16 out, size_t n, cudaStream_t s);
 int launch_split16_to_f32(CSplit16 in, float* out, size_t n, cudaStream_t s);
 

@@ -7,24 +7,11 @@ namespace cotr {
 namespace {
 
 // torchvision resnet stem: MaxPool2d(kernel 3, stride 2, padding 1) on NHWC, 8 channels per thread.
-// Dependency prologue / epilogue of the small kernels: hardware wait, or the counters of common.cuh (one polling thread)
-__device__ __forceinline__ void small_kernel_wait(const LaunchSync& y, int tile) {
-    if (threadIdx.x == 0) {
-        pdl_launch_dependents();
-        if (y.dep_mode != DEP_PDL) dep_wait_thread(y, tile);
-    }
-    if (y.dep_mode != DEP_PDL) __syncthreads(); else pdl_wait();
-}
-__device__ __forceinline__ void small_kernel_signal(const LaunchSync& y, int tile) {
-    if (y.sig == nullptr) return;
-    __syncthreads();
-    if (threadIdx.x == 0) dep_signal_thread(y, tile);
-}
-
-__global__ void maxpool_3x3s2_nhwc_kernel(const CSplit16 in, const Split16 out, int N, int H, int W, int C8, const LaunchSync sync) {
+__global__ void maxpool_3x3s2_nhwc_kernel(const CSplit16 in, const Split16 out, int N, int H, int W, int C8) {
     const int OH = H / 2, OW = W / 2;
     const size_t total = (size_t)N * OH * OW * C8;
-    small_kernel_wait(sync, 0);
+    if (threadIdx.x == 0) pdl_launch_dependents();
+    pdl_wait();
     for (size_t idx = blockIdx.x * (size_t)blockDim.x + threadIdx.x; idx < total;
          idx += (size_t)gridDim.x * blockDim.x) {
         const int c8 = idx % C8;
@@ -51,13 +38,13 @@ __global__ void maxpool_3x3s2_nhwc_kernel(const CSplit16 in, const Split16 out, 
         }
         store8_split(out, idx * 8, m);      // hi + lo is exact in fp32, so the re-split is lossless
     }
-    small_kernel_signal(sync, 0);
 }
 
 // The stem's operand (common.cuh "The stem's input"): fp32 (B,3,256,512) NCHW canvas -> per image n = 2*pair + half the
 // split16 NHWC4 copy with a zero border.  One thread per pixel: three coalesced channel reads, one 8-byte store per plane.
-__global__ void __launch_bounds__(256) stem_canvas_kernel(const float* __restrict__ img, const Split16 canvas, int n_img, const LaunchSync sync) {
-    small_kernel_wait(sync, 0);
+__global__ void __launch_bounds__(256) stem_canvas_kernel(const float* __restrict__ img, const Split16 canvas, int n_img) {
+    if (threadIdx.x == 0) pdl_launch_dependents();
+    pdl_wait();
     const size_t total = (size_t)n_img * 256 * 256;
     for (size_t idx = blockIdx.x * (size_t)blockDim.x + threadIdx.x; idx < total; idx += (size_t)gridDim.x * blockDim.x) {
         const int x = (int)(idx & 255), y = (int)((idx >> 8) & 255), n = (int)(idx >> 16);
@@ -70,7 +57,6 @@ __global__ void __launch_bounds__(256) stem_canvas_kernel(const float* __restric
         *reinterpret_cast<uint2*>(canvas.hi + off) = h;
         *reinterpret_cast<uint2*>(canvas.lo + off) = l;
     }
-    small_kernel_signal(sync, 0);
 }
 
 __device__ __forceinline__ float warp_sum(float v) {
@@ -124,11 +110,11 @@ __global__ void __launch_bounds__(256) ln_partials_kernel(const CSplit16 x, floa
 // out = LN_b(LN_a(x)), one warp per row (the decoder's last norm3 followed by decoder.norm)
 __global__ void __launch_bounds__(256) layernorm256_twice_kernel(const CSplit16 x, const float* __restrict__ g1, const float* __restrict__ b1,
                                                                  const float* __restrict__ g2, const float* __restrict__ b2,
-                                                                 const Split16 out, int rows, const LaunchSync sync) {
+                                                                 const Split16 out, int rows) {
     const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     const int lane = threadIdx.x & 31;
-    const int tile = (blockIdx.x * 8) >> 7;             // 8 rows per block: the 128-row tile they belong to
-    small_kernel_wait(sync, tile);
+    if (threadIdx.x == 0) pdl_launch_dependents();
+    pdl_wait();
     if (warp < rows) {
         const size_t off = (size_t)warp * kDModel + lane * 8;
         float v[8];
@@ -137,7 +123,6 @@ __global__ void __launch_bounds__(256) layernorm256_twice_kernel(const CSplit16 
         warp_layernorm256(v, g2, b2, lane);
         store8_split(out, off, v);
     }
-    small_kernel_signal(sync, tile);
 }
 
 template <bool F32_IN>
@@ -177,9 +162,10 @@ __global__ void __launch_bounds__(256) layernorm256_kernel(const CSplit16 x, con
 
 // position_encoding.py:41-45 with bases 1..64 on (x, y):
 // channel 2(k-1)+a = sin(fp32(k*pi) * p_a), channel 128 + 2(k-1)+a = cos(...).  Accurate sincosf: |angle| <= 64*pi.
-__global__ void __launch_bounds__(128) query_encode_kernel(const float* __restrict__ queries, const Split16 qpos, int rows, const LaunchSync sync) {
+__global__ void __launch_bounds__(128) query_encode_kernel(const float* __restrict__ queries, const Split16 qpos, int rows) {
     const int row = blockIdx.x;
-    small_kernel_wait(sync, row >> 7);
+    if (threadIdx.x == 0) pdl_launch_dependents();
+    pdl_wait();
     if (row >= rows) return;
     const int t = threadIdx.x;          // 0..127 = 2*(k-1) + axis
     const int k = (t >> 1) + 1;
@@ -195,7 +181,6 @@ __global__ void __launch_bounds__(128) query_encode_kernel(const float* __restri
     split_f16(c, h, l);
     qpos.hi[(size_t)row * kDModel + 128 + t] = h;
     qpos.lo[(size_t)row * kDModel + 128 + t] = l;
-    small_kernel_signal(sync, row >> 7);
 }
 
 __global__ void f32_to_split16_kernel(const float* __restrict__ in, const Split16 out, size_t n) {
@@ -218,10 +203,10 @@ int grid_for(size_t total, int block) {
 
 }  // namespace
 
-int launch_maxpool_3x3s2_nhwc(CSplit16 in, Split16 out, int N, int H, int W, int C, cudaStream_t s, LaunchSync sync) {
+int launch_maxpool_3x3s2_nhwc(CSplit16 in, Split16 out, int N, int H, int W, int C, cudaStream_t s) {
     COTR_CHECK((C & 7) == 0 && (H & 1) == 0 && (W & 1) == 0, "maxpool: unsupported shape");
     const size_t total = (size_t)N * (H / 2) * (W / 2) * (C / 8);
-    COTR_CHECK_CUDA(launch_kernel(maxpool_3x3s2_nhwc_kernel, dim3(grid_for(total, 256)), dim3(256), 0, s, in, out, N, H, W, C / 8, sync));
+    COTR_CHECK_CUDA(launch_kernel(maxpool_3x3s2_nhwc_kernel, dim3(grid_for(total, 256)), dim3(256), 0, s, in, out, N, H, W, C / 8));
     return 0;
 }
 
@@ -238,10 +223,9 @@ int launch_ln_partials(CSplit16 x, float2* part, int rows, cudaStream_t s) {
     return 0;
 }
 
-int launch_layernorm_twice(CSplit16 x, const float* g1, const float* b1, const float* g2, const float* b2, Split16 out, int rows, cudaStream_t s,
-                           LaunchSync sync) {
+int launch_layernorm_twice(CSplit16 x, const float* g1, const float* b1, const float* g2, const float* b2, Split16 out, int rows, cudaStream_t s) {
     if (rows <= 0) return 0;
-    COTR_CHECK_CUDA(launch_kernel(layernorm256_twice_kernel, dim3((rows + 7) / 8), dim3(256), 0, s, x, g1, b1, g2, b2, out, rows, sync));
+    COTR_CHECK_CUDA(launch_kernel(layernorm256_twice_kernel, dim3((rows + 7) / 8), dim3(256), 0, s, x, g1, b1, g2, b2, out, rows));
     return 0;
 }
 
@@ -251,15 +235,15 @@ int launch_layernorm_f32(const float* x, const float* gamma, const float* beta, 
     return 0;
 }
 
-int launch_query_encode(const float* queries, Split16 qpos, int rows, cudaStream_t s, LaunchSync sync) {
+int launch_query_encode(const float* queries, Split16 qpos, int rows, cudaStream_t s) {
     if (rows <= 0) return 0;
-    COTR_CHECK_CUDA(launch_kernel(query_encode_kernel, dim3(rows), dim3(128), 0, s, queries, qpos, rows, sync));
+    COTR_CHECK_CUDA(launch_kernel(query_encode_kernel, dim3(rows), dim3(128), 0, s, queries, qpos, rows));
     return 0;
 }
 
-int launch_stem_canvas(const float* img, Split16 canvas, int n_img, cudaStream_t s, LaunchSync sync) {
+int launch_stem_canvas(const float* img, Split16 canvas, int n_img, cudaStream_t s) {
     if (n_img <= 0) return 0;
-    COTR_CHECK_CUDA(launch_kernel(stem_canvas_kernel, dim3(grid_for((size_t)n_img * 256 * 256, 256)), dim3(256), 0, s, img, canvas, n_img, sync));
+    COTR_CHECK_CUDA(launch_kernel(stem_canvas_kernel, dim3(grid_for((size_t)n_img * 256 * 256, 256)), dim3(256), 0, s, img, canvas, n_img));
     return 0;
 }
 

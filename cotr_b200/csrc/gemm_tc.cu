@@ -43,8 +43,6 @@ namespace cotr {
 
 int g_tc_variant = 0;                   // bring-up switch (reserved)
 int g_use_pdl = 1;                      // programmatic dependent launch (common.cuh); cotr_debug_set_variant bit 8 clears it
-long long* g_tc_timestamps = nullptr;   // debug: 64 clock64() stamps per CTA (cotr_debug_set_timestamps), else null
-int g_tc_trace_idx = 0;                 // trace mode: launch counter (common.cuh next_trace_block)
 
 namespace {
 
@@ -115,16 +113,12 @@ struct EpiOperands {
     uint4 res_hi[2], res_lo[2];
 };
 
-// DLN: the instantiation carries the deferred-LayerNorm operands (GemmParams::a_ln_cs / res_ln_part / ln_part_out) and the
-// dataflow dependencies (GemmParams::sync).  The default schedule uses DLN = false kernels, which contain none of it.
+// DLN: the instantiation carries the deferred-LayerNorm operands (GemmParams::a_ln_cs / res_ln_part / ln_part_out).
+// The default schedule uses DLN = false kernels, which contain none of it.
 template <int BN, bool LN, int MODE, bool DLN>
-__global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const GemmParams p, const int npad, long long* __restrict__ ts) {
+__global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const GemmParams p, const int npad) {
     using C = Cfg<BN>;
     constexpr int BM = C::BM;
-    // debug timeline (ts != null): 64 clock64() stamps per CTA (COTR_TS slots below)
-    long long* my_ts = ts ? ts + (size_t)((blockIdx.z * gridDim.y + blockIdx.y) * gridDim.x + blockIdx.x) * 64 : nullptr;
-    const long long t_start = ts ? clock64() : 0;
-#define COTR_TS(slot) do { if (my_ts) my_ts[(slot)] = clock64() - t_start; } while (0)
     extern __shared__ uint8_t smem_raw[];
     const uint32_t raw_addr = smem_u32(smem_raw);
     uint8_t* stage_base = smem_raw + (((raw_addr + 1023u) & ~1023u) - raw_addr);      // SWIZZLE_128B needs 1024-byte alignment
@@ -133,15 +127,13 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const GemmParams p
     uint64_t* empty = bars + C::kStages;
     uint64_t* part_full = bars + 2 * C::kStages;           // split-K leader: all peers' partial tiles have landed
     uint64_t* vec_full = bars + 2 * C::kStages + 1;        // deferred LayerNorm: the per-column vectors are staged
-    uint64_t* dep_ready = bars + 2 * C::kStages + 2;       // dataflow mode: the polling thread has seen the producer's counters
-    const bool dflow = DLN && p.sync.dep_mode != DEP_PDL;  // counters in global memory instead of griddepcontrol.wait (common.cuh)
     float* vec_a = reinterpret_cast<float*>(stage_base + C::kVecOffset);      // a_ln: column sums of W'; res_ln: gamma
     float* vec_b = vec_a + BN;                                                  //                         res_ln: beta
     float2* st_a = reinterpret_cast<float2*>(vec_b + BN);                       // (mean, rstd) of the A rows of this tile
     float2* st_r = st_a + BM;                                                   // (mean, rstd) of the residual rows
     float* acc_tile = reinterpret_cast<float*>(stage_base);                     // epilogue: summed accumulators [BM][kAccPitch]
     // deferred LayerNorm (GemmParams::a_ln_cs / res_ln_part / ln_part_out): only the row-major loader instantiations carry it
-    static_assert(!DLN || (MODE == LD_GATHER && !LN), "deferred LayerNorm / dataflow: row-major operand tiles only");
+    static_assert(!DLN || (MODE == LD_GATHER && !LN), "deferred LayerNorm: row-major operand tiles only");
     constexpr bool kCanLnA = DLN;
     const bool has_aln = kCanLnA && p.a_ln_cs != nullptr;
     const bool stage_vec = kCanLnA && !LN && (has_aln || p.res_ln_part != nullptr);
@@ -165,17 +157,13 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const GemmParams p
             mbar_init(&empty[s], 8);          // one arrival per consumer warp
         }
         mbar_init(part_full, 1);
-        if (DLN) {
-            mbar_init(vec_full, 64);
-            mbar_init(dep_ready, 1);
-        }
+        if (DLN) mbar_init(vec_full, 64);
         mbar_fence_init();
         if (ksplit > 1) mbar_arrive_expect_tx(part_full, (uint32_t)(ksplit - 1) * (uint32_t)(BM / ksplit) * C::kPartPitch);
     }
     __syncthreads();
     // split-K: tell the cluster that this CTA runs and its barriers exist (waited for just before the first remote access)
     if (ksplit > 1) cluster_arrive();
-    if (threadIdx.x == 0) COTR_TS(1);
 
     if (warp >= 8) {
         // ================= producer warpgroup: A tile by cp.async, weights by bulk TMA ============================
@@ -217,17 +205,14 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const GemmParams p
         if (t == 0) {
             for (int it = 0; it < KC && it < C::kStages; ++it) load_weights(it);
             pdl_launch_dependents();
-            if (dflow) { dep_wait_thread(p.sync, blockIdx.x); mbar_arrive(dep_ready); }
         }
-        if (dflow) mbar_wait(dep_ready, 0); else pdl_wait();
-        if (t == 0) COTR_TS(2);
+        pdl_wait();
 
 #pragma unroll 1
         for (int it = 0; it < KC; ++it) {
             const int s = it % C::kStages;
             const uint32_t ph = (uint32_t)(it / C::kStages) & 1u;
             mbar_wait(&empty[s], ph ^ 1u);
-            if (t == 0 && it < 8) COTR_TS(3 + 2 * it);
             if (t == 0 && it >= C::kStages) load_weights(it);
             const int k0 = (it0 + it) * BK;
             {
@@ -260,7 +245,6 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const GemmParams p
                 }
                 cp_async_mbar_arrive_noinc(&full_a[s]);
             }
-            if (t == 0 && it < 8) COTR_TS(4 + 2 * it);
         }
 
         if (stage_vec && warp >= 10) {
@@ -341,7 +325,6 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const GemmParams p
             const uint32_t ph = (uint32_t)(it / C::kStages) & 1u;
             mbar_wait(&full_a[s], ph);
             fence_proxy_async_smem();                          // cp.async (generic proxy) data -> wgmma (async proxy)
-            if (threadIdx.x == 0 && it < 8) COTR_TS(24 + 2 * it);
             const uint32_t a_addr = smem_u32(stage_base + (size_t)s * C::kStage);
             const uint32_t b_addr = a_addr + 2 * C::kAPlane;
             fence_all();
@@ -361,11 +344,9 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const GemmParams p
             wgmma_wait<1>();                                   // the previous chunk's MMAs have read their stage
             fence_all();
             if (it > 0 && lane == 0) mbar_arrive(&empty[(it - 1) % C::kStages]);
-            if (threadIdx.x == 0 && it < 8) COTR_TS(25 + 2 * it);
         }
         wgmma_wait<0>();
         fence_all();
-        if (threadIdx.x == 0) COTR_TS(41);
         // park the sums (corrections first, then the main slots, RN adds) as an fp32 tile once both warpgroups are done
         // with the stages.  Fragment of m64nWN: register 4 j + {0,1} = row (warp % 4) * 16 + lane / 4, columns
         // 8 j + 2 (lane % 4) + {0,1}; registers 4 j + {2,3} = the same columns 8 rows further down.
@@ -397,7 +378,7 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const GemmParams p
     const int half = warp >> 2;              // column half of the tile it handles
     if (ksplit > 1) cluster_wait();          // every CTA of the cluster has started (long ago by now)
     if (warp < 8 && half < C::kEpiHalves && ew * 32 < BM) {
-        if (dflow) mbar_wait(dep_ready, 0); else pdl_wait();      // residual / add operands come from the previous kernels
+        pdl_wait();                          // residual / add operands come from the previous kernels
         const int cbeg = half * C::kChunksW * 16;
         const int row = m0 + ew * 32 + lane;
         // split-K: row group q is finished by CTA q * ksplit / 4; the other CTAs only contribute partial sums
@@ -576,7 +557,6 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const GemmParams p
             if (has_aln) a_st = st_a[ew * 32 + lane];
             if (res_ln) { res_st = st_r[ew * 32 + lane]; res_shift = -res_st.x * res_st.y; }
         }
-        if (threadIdx.x == 0) COTR_TS(20);
         // Narrow tiles read their own accumulators into registers right away: senders push them, owners overlap the
         // shared-memory reads with the wait for the peers' partial rows.
         constexpr bool kPreload = !LN && C::kChunksW <= 2;
@@ -601,11 +581,8 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const GemmParams p
                     for (int j = 0; j < 16; j += 4)
                         st_async_f32x4(remote + (((uint32_t)((c + j) >> 2) ^ part_swz) << 4), v[j], v[j + 1], v[j + 2], v[j + 3], remote_bar);
                 }
-                if (threadIdx.x == 0) COTR_TS(22);
             } else {
-                if (threadIdx.x == 0) COTR_TS(22);
                 mbar_wait(part_full, 0);             // (ksplit - 1) x (128 / ksplit) rows x BN floats have landed
-                if (threadIdx.x == 0) COTR_TS(23);
             }
         }
         if (mine) {
@@ -623,7 +600,6 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const GemmParams p
                 } else {
                     load_acc(c, v);
                 }
-                if (threadIdx.x == 0 && ci < 2) COTR_TS(30 + 4 * ci);
                 if (BN > 16 || !tail) {                          // (a ragged N only exists in the 16-wide instantiation)
                     apply(ops[ci % C::kRing], v, nb);
                 } else {
@@ -646,12 +622,9 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const GemmParams p
                     for (int j = 0; j < 16; ++j) { const float d = v[j] - sm; m2 = fmaf(d, d, m2); }
                     p.ln_part_out[(size_t)row * 16 + (nb >> 4)] = make_float2(sm, m2);
                 }
-                if (threadIdx.x == 0 && ci < 2) COTR_TS(31 + 4 * ci);
                 emit16(c, v);
-                if (threadIdx.x == 0 && ci < 2) COTR_TS(32 + 4 * ci);
                 if (ci + C::kRing < C::kChunksW) prefetch(nb + 16 * C::kRing, ops[ci % C::kRing]);
             }
-            if (threadIdx.x == 0) COTR_TS(38);
             drain();
         } else {
             // fused residual + LayerNorm (eps 1e-5, biased variance) over the 256 columns this thread owns.  One pass
@@ -702,17 +675,11 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const GemmParams p
             drain();
         }
         }   // leader / unsplit epilogue
-        if (threadIdx.x == 0) COTR_TS(21);
     }
 
+    // the producer warps leave with the rest of the CTA, after the consumers have seen all of their copies land
     __syncthreads();
-    if (DLN && threadIdx.x == 0) dep_signal_thread(p.sync, blockIdx.x);       // every store of this CTA precedes the barrier above
-    if (threadIdx.x == 0) COTR_TS(60);
-    if (my_ts && threadIdx.x == 0) my_ts[62] = global_ns();
-#undef COTR_TS
 }
-
-thread_local GemmLaunchInfo* g_launch_info = nullptr;       // where launch_one reports the grid it chose
 
 template <int BN, bool LN, int MODE, bool DLN = false>
 int launch_one(const GemmParams& p, cudaStream_t s) {
@@ -737,13 +704,12 @@ int launch_one(const GemmParams& p, cudaStream_t s) {
     }
     COTR_CHECK(p.a_ln_cs == nullptr || (DLN && p.K == 256 && p.a_mode == A_ROWMAJOR && p.a_ln_part != nullptr),
                "gemm_tc: the deferred LayerNorm on A needs a row-major operand with K = 256 and its partial statistics");
-    COTR_CHECK((p.res_ln_part == nullptr && p.ln_part_out == nullptr && p.sync.dep_mode == DEP_PDL && p.sync.sig == nullptr) || DLN,
+    COTR_CHECK((p.res_ln_part == nullptr && p.ln_part_out == nullptr) || DLN,
                "gemm_tc: deferred-LayerNorm residual / statistics on an unsupported tile");
     COTR_CHECK(p.ln_part_out == nullptr || (p.N == 256 && !p.remap && p.out_f32 == nullptr), "gemm_tc: row statistics need a plain N = 256 output");
     grid.z = ksplit;
     const size_t smem = C::kSmemBytes + (size_t)(ksplit - 1) * (C::BM / ksplit) * C::kPartPitch;     // incoming partial rows
-    if (g_launch_info) *g_launch_info = GemmLaunchInfo{(int)grid.x, (int)grid.y, ksplit};
-    COTR_CHECK_CUDA(launch_kernel_cluster(gemm_tc_kernel<BN, LN, MODE, DLN>, grid, dim3(kThreads), smem, s, ksplit, p, npad, next_trace_block()));
+    COTR_CHECK_CUDA(launch_kernel_cluster(gemm_tc_kernel<BN, LN, MODE, DLN>, grid, dim3(kThreads), smem, s, ksplit, p, npad));
     return 0;
 }
 
@@ -752,8 +718,7 @@ int launch_mode(const GemmParams& p, cudaStream_t s) {
     const bool gather = (p.a_mode == A_ROWMAJOR || p.a_mode == A_TOKENS);
     if (gather && (p.K & 7) == 0 && (p.lda & 7) == 0) {
         if constexpr (!LN) {
-            const bool dln = p.a_ln_cs != nullptr || p.res_ln_part != nullptr || p.ln_part_out != nullptr ||
-                             p.sync.dep_mode != DEP_PDL || p.sync.sig != nullptr;
+            const bool dln = p.a_ln_cs != nullptr || p.res_ln_part != nullptr || p.ln_part_out != nullptr;
             if (dln) return launch_one<BN, LN, LD_GATHER, true>(p, s);
         }
         return launch_one<BN, LN, LD_GATHER>(p, s);
@@ -842,11 +807,7 @@ float tc_pack_weight(const float* w, int N, int K, void* dst_host) {
     return ldexpf(1.f, -e);
 }
 
-int launch_gemm_tc(const GemmParams& p, cudaStream_t s, GemmLaunchInfo* info) {
-    struct InfoScope {          // launch_one fills *info through the thread-local pointer
-        explicit InfoScope(GemmLaunchInfo* i) { g_launch_info = i; }
-        ~InfoScope() { g_launch_info = nullptr; }
-    } scope(info);
+int launch_gemm_tc(const GemmParams& p, cudaStream_t s) {
     COTR_CHECK(p.M > 0 && p.N > 0 && p.K > 0, "gemm_tc: empty problem %d x %d x %d", p.M, p.N, p.K);
     COTR_CHECK(p.Wtc != nullptr, "gemm_tc: weight has no tensor-core image");
     COTR_CHECK(p.out_f32 != nullptr || (p.N & 15) == 0, "gemm_tc: split16 outputs need N %% 16 == 0 (N=%d)", p.N);

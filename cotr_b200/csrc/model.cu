@@ -15,7 +15,6 @@
 namespace cotr {
 
 extern int g_tc_variant;
-extern long long* g_tc_timestamps;
 static thread_local char g_error[1024] = "";
 
 void set_error(const char* fmt, ...) {
@@ -84,9 +83,7 @@ struct Workspace {
     Split16 canvas = kNoSplit, stem = kNoSplit, bx = kNoSplit, by = kNoSplit, bt1 = kNoSplit, bt2 = kNoSplit, bds = kNoSplit;
     // encoder
     Split16 src = kNoSplit, xa = kNoSplit, xb = kNoSplit, qk = kNoSplit, vt = kNoSplit, ao = kNoSplit, ffh = kNoSplit;
-    Split16 qk2 = kNoSplit, vt2 = kNoSplit;      // odd encoder layers: with tile-level dependencies layer l+1 projects while layer l still attends
-    unsigned char *kvimg = nullptr, *kvimg2 = nullptr;      // [pairs][8 heads] attention operand images of the encoder's own k / v
-    int* sync_ctr = nullptr;      // dataflow counter blocks (common.cuh LaunchSync): kSyncBlocks x kSyncBlockInts ints
+    unsigned char* kvimg = nullptr;      // [pairs][8 heads] attention operand images of the encoder's own k / v
     float* ln_tmp = nullptr;      // fp32 [tokens][256]: pre-LayerNorm rows of the SIMT cross-check path
     float2 *enc_st_a = nullptr, *enc_st_b = nullptr;     // [tokens][16] partial row statistics of xa / xb (deferred LayerNorms)
     // decoder
@@ -307,57 +304,10 @@ std::vector<float> grid_position_table() {
 // ----------------------------------------------------------------------------------------------
 // launch helpers (all kernel launches of the forward go through these, so they can be counted / profiled)
 // ----------------------------------------------------------------------------------------------
-// Dataflow dependencies between the launches of one call (common.cuh LaunchSync): the planner hands every launch the
-// counter block of its predecessor (what to wait for) and a fresh block of its own (where to announce its tiles).
-struct SyncPlan {
-    int* base = nullptr;       // counter blocks of this call (zeroed by the caller)
-    int cap_blocks = 0;
-    int next = 0;
-    bool on = false;
-    const int* prev = nullptr;             // the previous launch's block; null: it announced nothing -> hardware wait
-    int prev_total = 0, prev_tile_target = 0, prev_tiles = 0, prev_rows = -1;
-};
-
 struct Run {
     cotr_model* m;
     cudaStream_t s;
-    SyncPlan* sp = nullptr;
 };
-
-// mode: what this launch would like to wait for (degraded to DEP_ALL when the producer's row tiling does not match);
-// rows: size of this launch's row space; returns the LaunchSync with the dependency part and the signal block filled.
-LaunchSync plan_dep(const Run& r, int mode, int rows, int span = 0) {
-    LaunchSync y;
-    memset(&y, 0, sizeof(y));
-    SyncPlan* sp = r.sp;
-    if (!sp || !sp->on) return y;
-    if (sp->prev) {
-        const bool tile_ok = sp->prev_tiles > 0 && sp->prev_rows == rows;
-        y.dep = sp->prev;
-        if (mode == DEP_TILE && tile_ok) { y.dep_mode = DEP_TILE; y.dep_target = sp->prev_tile_target; }
-        else if (mode == DEP_SPAN && tile_ok && span > 0 && sp->prev_tiles % span == 0) { y.dep_mode = DEP_SPAN; y.dep_span = span; y.dep_target = sp->prev_tile_target; }
-        else { y.dep_mode = DEP_ALL; y.dep_target = sp->prev_total; }
-    }
-    if (sp->next < sp->cap_blocks) {
-        y.sig = sp->base + (size_t)sp->next * kSyncBlockInts;
-        sp->next++;
-    }
-    return y;
-}
-// after the launch: what the NEXT launch may wait for
-void plan_done(const Run& r, const LaunchSync& y, int total, int tile_target, int rows) {
-    SyncPlan* sp = r.sp;
-    if (!sp || !sp->on) return;
-    sp->prev = y.sig;
-    sp->prev_total = total;
-    sp->prev_tile_target = tile_target;
-    sp->prev_tiles = y.sig ? y.sig_tiles : 0;
-    sp->prev_rows = rows;
-}
-inline int sync_tiles_for(int rows) {          // per-tile counters only while they fit the block
-    const int t = (rows + 127) / 128;
-    return t <= kSyncBlockInts - 1 ? t : 0;
-}
 
 enum KernelId { K_GEMM_TC = 0, K_GEMM_SIMT = 1, K_ATTN_TC = 2, K_ATTN_SIMT = 3, K_LAYERNORM = 4, K_MAXPOOL = 5, K_QENC = 6, K_STEM_CANVAS = 7 };
 
@@ -397,25 +347,14 @@ GemmParams gemm_base(int M, int N, int K, CSplit16 A, int lda, const float* W, c
     return p;
 }
 
-// One tensor-core GEMM launch with its dataflow bookkeeping.  dep_mode: DEP_ALL / DEP_TILE (the A rows of a CTA's tile come
-// from the same 128-row tile of the previous launch, and nothing this launch overwrites is still read by other tiles).
-int launch_tc(const Run& r, GemmParams& p, int dep_mode = DEP_ALL) {
-    // only the row-major operand kernels exist in a dataflow-capable form (gemm_tc.cu, DLN instantiations): convolutions
-    // keep the hardware wait and announce nothing, so their successor falls back to the hardware wait as well
-    const bool flow_ok = (p.a_mode == A_ROWMAJOR || p.a_mode == A_TOKENS) && (p.K & 7) == 0 && (p.lda & 7) == 0;
-    if (flow_ok) p.sync = plan_dep(r, dep_mode, p.M);
-    else if (r.sp) r.sp->prev = nullptr;
-    p.sync.sig_tiles = p.sync.sig ? sync_tiles_for(p.M) : 0;
-    GemmLaunchInfo info{0, 0, 1};
+int launch_tc(const Run& r, const GemmParams& p) {
     LaunchScope scope(r, K_GEMM_TC, p.M, p.N, p.K);
-    if (launch_gemm_tc(p, r.s, &info)) return 1;
-    if (flow_ok) plan_done(r, p.sync, info.row_tiles * info.col_tiles * info.ksplit, info.col_tiles * info.ksplit, p.M);
-    return 0;
+    return launch_gemm_tc(p, r.s);
 }
 
 // ln_scratch: fp32 [M][256] staging for the SIMT path (the tensor-core GEMM fuses LayerNorm into its epilogue).
-int run_gemm(const Run& r, GemmParams p, float* ln_scratch, int dep_mode = DEP_ALL) {
-    if (r.m->gemm_path == 0 && p.ln_gamma == nullptr) return launch_tc(r, p, dep_mode);
+int run_gemm(const Run& r, GemmParams p, float* ln_scratch) {
+    if (r.m->gemm_path == 0 && p.ln_gamma == nullptr) return launch_tc(r, p);
     if (r.m->gemm_path == 0) {
         // The fused LayerNorm epilogue needs the whole 256-wide row in one CTA (128 x 256 tile): with few rows that is
         // a handful of CTAs doing a long serial epilogue while the other SMs idle.  Below ~64 row tiles the GEMM runs
@@ -424,12 +363,7 @@ int run_gemm(const Run& r, GemmParams p, float* ln_scratch, int dep_mode = DEP_A
         const float* g = p.ln_gamma;
         const float* b = p.ln_beta;
         if (defuse) { p.ln_gamma = nullptr; p.ln_beta = nullptr; }
-        // (legacy schedule, not used by the deferred-LayerNorm forward: no dataflow announcements)
-        if (r.sp) r.sp->prev = nullptr;
-        {
-            LaunchScope scope(r, K_GEMM_TC, p.M, p.N, p.K);
-            if (launch_gemm_tc(p, r.s)) return 1;
-        }
+        if (launch_tc(r, p)) return 1;
         if (defuse) {
             LaunchScope scope(r, K_LAYERNORM, p.M, kDModel, 0);
             if (launch_layernorm(cs(p.out), g, b, p.out, p.M, r.s)) return 1;
@@ -455,14 +389,14 @@ int run_gemm(const Run& r, GemmParams p, float* ln_scratch, int dep_mode = DEP_A
 
 int run_linear(const Run& r, const DevLinear& L, int M, CSplit16 A, int lda, Split16 out, int ldc, bool relu,
                CSplit16 residual = CSplit16{nullptr, nullptr}, int ldr = 0, const float* ln_g = nullptr,
-               const float* ln_b = nullptr, float* ln_scratch = nullptr, int dep_mode = DEP_ALL) {
+               const float* ln_b = nullptr, float* ln_scratch = nullptr) {
     // explicit-LayerNorm schedule: layers that also exist in a gamma-folded form use their plain image here
     GemmParams p = gemm_base(M, L.n, L.k, A, lda, L.w, L.wtc_plain ? L.wtc_plain : L.wtc, L.wtc_plain ? L.wtc_plain_scale : L.wtc_scale, out, ldc);
     p.bias = L.b;
     p.relu = relu ? 1 : 0;
     p.res = residual; p.ldr = ldr;
     p.ln_gamma = ln_g; p.ln_beta = ln_b;
-    return run_gemm(r, p, ln_scratch, dep_mode);
+    return run_gemm(r, p, ln_scratch);
 }
 
 // Tensor-core path only: linear layer with deferred LayerNorms (GemmParams::a_ln_cs / res_ln_part / ln_part_out).
@@ -471,7 +405,7 @@ int run_linear(const Run& r, const DevLinear& L, int M, CSplit16 A, int lda, Spl
 //   res_part   non-null: the residual operand is a deferred LayerNorm (res_g, res_b) of the stored rows
 int run_linear_dln(const Run& r, const DevLinear& L, int M, CSplit16 A, int lda, Split16 out, int ldc, bool relu,
                    const float2* a_part, float2* part_out, CSplit16 residual = CSplit16{nullptr, nullptr}, int ldr = 0,
-                   const float2* res_part = nullptr, const float* res_g = nullptr, const float* res_b = nullptr, int dep_mode = DEP_TILE) {
+                   const float2* res_part = nullptr, const float* res_g = nullptr, const float* res_b = nullptr) {
     GemmParams p = gemm_base(M, L.n, L.k, A, lda, L.w, L.wtc, L.wtc_scale, out, ldc);
     p.bias = a_part ? L.b_tc : L.b;
     p.relu = relu ? 1 : 0;
@@ -479,7 +413,7 @@ int run_linear_dln(const Run& r, const DevLinear& L, int M, CSplit16 A, int lda,
     if (a_part) { p.a_ln_cs = L.cs; p.a_ln_part = a_part; }
     p.ln_part_out = part_out;
     p.res_ln_part = res_part; p.res_ln_gamma = res_g; p.res_ln_beta = res_b;
-    return launch_tc(r, p, dep_mode);
+    return launch_tc(r, p);
 }
 
 int run_conv(const Run& r, const DevConv& c, int n_img, CSplit16 in, int H, int W, Split16 out, bool relu, CSplit16 residual) {
@@ -501,23 +435,11 @@ int run_conv(const Run& r, const DevConv& c, int n_img, CSplit16 in, int H, int 
     return run_gemm(r, p, nullptr);
 }
 
-// dep_mode / span: DEP_TILE (decoder: a CTA reads only its own 128 query rows from the previous launch) or DEP_SPAN
-// (encoder: the keys and values of the whole pair, `span` row tiles); both need query tiles aligned with 128-row tiles
-int run_attention(const Run& r, AttnParams p, int dep_mode = DEP_ALL, int span = 0) {
+int run_attention(const Run& r, const AttnParams& p) {
     // recorded as M = query rows, N = 512 keys, K = 32 x 8 heads
-    const int rows = p.nq * p.npairs;
-    LaunchScope scope(r, r.m->gemm_path == 0 ? K_ATTN_TC : K_ATTN_SIMT, rows, kTokens, kDModel);
+    LaunchScope scope(r, r.m->gemm_path == 0 ? K_ATTN_TC : K_ATTN_SIMT, p.nq * p.npairs, kTokens, kDModel);
     if (r.m->gemm_path != 0) return launch_attention_simt(p, r.s);
-    if (p.nq < 32) {                          // launch_attention_tc hands these to the SIMT kernel: hardware wait, no announcements
-        if (r.sp) r.sp->prev = nullptr;
-        return launch_attention_tc(p, r.s);
-    }
-    const bool aligned = (p.nq % 128) == 0;
-    p.sync = plan_dep(r, aligned ? dep_mode : DEP_ALL, rows, span);
-    p.sync.sig_tiles = (p.sync.sig && aligned) ? sync_tiles_for(rows) : 0;
-    if (launch_attention_tc(p, r.s)) return 1;
-    plan_done(r, p.sync, ((p.nq + 127) / 128) * kHeads * p.npairs, kHeads, rows);
-    return 0;
+    return launch_attention_tc(p, r.s);
 }
 
 // ----------------------------------------------------------------------------------------------
@@ -531,8 +453,8 @@ constexpr size_t kT2Elems = 64 * 64 * 64;          // largest conv2 output per i
 size_t encode_ws_elems(int B) {
     const size_t img = 2 * (size_t)B;
     const size_t tok = (size_t)B * kTokens;
-    return img * (kStemCanvasElems + kStemElems + 3 * kBigElems + kT1Elems + kT2Elems) + tok * (kDModel * 4 + 4 * kDModel + kFF) +
-           2 * (size_t)B * kVtLayer + tok * kDModel /* fp32 LN scratch */ + tok * 64 /* row statistics */;
+    return img * (kStemCanvasElems + kStemElems + 3 * kBigElems + kT1Elems + kT2Elems) + tok * (kDModel * 4 + 2 * kDModel + kFF) +
+           (size_t)B * kVtLayer + tok * kDModel /* fp32 LN scratch */ + tok * 64 /* row statistics */;
 }
 size_t decode_ws_elems(int rows) {
     return (size_t)rows * (kDModel * 8 + kQpCols + kFF) + (size_t)rows * kDModel /* fp32 LN scratch */ + (size_t)rows * 64 /* row statistics */;
@@ -553,30 +475,15 @@ int ws_alloc_f32(float** p, size_t elems) {
 }
 void ws_free_f32(float** p) { if (*p) { cudaFree(*p); *p = nullptr; } }
 
-// Dataflow counters: kSyncEncodeBlocks for cotr_encode_context, kSyncChunkBlocks per decoder chunk behind them.
-constexpr int kSyncEncodeBlocks = 128;
-constexpr int kSyncChunkBlocks = 48;
-constexpr int kSyncBlocks = 1024;
-
-int ensure_sync_ctr(cotr_model* m) {
-    if (m->ws.sync_ctr) return 0;
-    COTR_CHECK_CUDA(cudaMalloc((void**)&m->ws.sync_ctr, (size_t)kSyncBlocks * kSyncBlockInts * sizeof(int)));
-    return 0;
-}
-// bring-up switch: cotr_debug_set_variant bit 18 turns the dataflow dependencies off (hardware griddepcontrol.wait everywhere)
 // Schedule selection.
 // Deferred LayerNorm (no LayerNorm launches; consumers normalise on the fly) removes 12 launches from the encoder and
 // 12 from each decoder chunk but makes its consumer GEMMs a little longer: it pays off only once a section has
-// thousands of rows (the launches saved then outweigh the longer epilogues), so each section picks it by its row count.  cotr_debug_set_variant overrides: bit 19 = always deferred, bit 16 = never.  Bits 19 + 18 together
-// additionally swap griddepcontrol.wait for the counter-based dataflow dependencies of common.cuh - measured slower
-// everywhere, opt-in only.
+// thousands of rows (the launches saved then outweigh the longer epilogues), so each section picks it by its row count.
+// cotr_debug_set_variant overrides: bit 19 = always deferred, bit 16 = never.
 constexpr int kDeferredLnMinRows = 2048;
 inline bool deferred_ln_enabled(const cotr_model* m, int rows) {
     if (m->gemm_path != 0 || (g_tc_variant & (1 << 16))) return false;
     return (g_tc_variant & (1 << 19)) != 0 || rows >= kDeferredLnMinRows;
-}
-inline bool dataflow_enabled(const cotr_model* m) {
-    return m->gemm_path == 0 && (g_tc_variant & (1 << 18)) != 0 && (g_tc_variant & (1 << 19)) != 0 && !(g_tc_variant & (1 << 16)) && g_use_pdl;
 }
 
 // Captured graphs embed workspace / staging / context addresses: whenever one of those is reallocated every graph is
@@ -608,11 +515,10 @@ int ensure_encode_ws(cotr_model* m, int B) {
     if (B <= w.cap_pairs) return 0;
     COTR_CHECK_CUDA(cudaDeviceSynchronize());
     drop_graphs(m);
-    Split16* bufs[] = {&w.canvas, &w.stem, &w.bx, &w.by, &w.bt1, &w.bt2, &w.bds, &w.src, &w.xa, &w.xb, &w.qk, &w.vt, &w.ao, &w.ffh, &w.qk2, &w.vt2};
+    Split16* bufs[] = {&w.canvas, &w.stem, &w.bx, &w.by, &w.bt1, &w.bt2, &w.bds, &w.src, &w.xa, &w.xb, &w.qk, &w.vt, &w.ao, &w.ffh};
     for (Split16* b : bufs) ws_free(b);
     ws_free_f32(&w.ln_tmp);
     if (w.kvimg) { cudaFree(w.kvimg); w.kvimg = nullptr; }
-    if (w.kvimg2) { cudaFree(w.kvimg2); w.kvimg2 = nullptr; }
     ws_free_f32(reinterpret_cast<float**>(&w.enc_st_a));
     ws_free_f32(reinterpret_cast<float**>(&w.enc_st_b));
     const size_t img = 2 * (size_t)B, tok = (size_t)B * kTokens;
@@ -620,15 +526,12 @@ int ensure_encode_ws(cotr_model* m, int B) {
         ws_alloc(&w.bds, img * kBigElems) || ws_alloc(&w.bt1, img * kT1Elems) || ws_alloc(&w.bt2, img * kT2Elems) ||
         ws_alloc(&w.src, tok * kDModel) || ws_alloc(&w.xa, tok * kDModel) || ws_alloc(&w.xb, tok * kDModel) ||
         ws_alloc(&w.qk, tok * 2 * kDModel) || ws_alloc(&w.vt, (size_t)B * kVtLayer) || ws_alloc(&w.ao, tok * kDModel) ||
-        ws_alloc(&w.qk2, tok * 2 * kDModel) || ws_alloc(&w.vt2, (size_t)B * kVtLayer) ||
         ws_alloc(&w.ffh, tok * kFF) || ws_alloc_f32(&w.ln_tmp, tok * kDModel) ||
         ws_alloc_f32(reinterpret_cast<float**>(&w.enc_st_a), tok * 32) || ws_alloc_f32(reinterpret_cast<float**>(&w.enc_st_b), tok * 32))
         return 1;
     COTR_CHECK_CUDA(cudaMalloc((void**)&w.kvimg, (size_t)B * kHeads * kAttnHeadImgBytes));
-    COTR_CHECK_CUDA(cudaMalloc((void**)&w.kvimg2, (size_t)B * kHeads * kAttnHeadImgBytes));
     // the 16 pad bytes of every value key group are copied by the bulk TMA: keep them defined
     COTR_CHECK_CUDA(cudaMemset(w.kvimg, 0, (size_t)B * kHeads * kAttnHeadImgBytes));
-    COTR_CHECK_CUDA(cudaMemset(w.kvimg2, 0, (size_t)B * kHeads * kAttnHeadImgBytes));
     // the border of the stem canvas is the convolution's zero padding: written here, never again
     COTR_CHECK_CUDA(cudaMemset(w.canvas.hi, 0, img * kStemCanvasElems * 2 * sizeof(__half)));
     w.cap_pairs = B;
@@ -664,14 +567,9 @@ int encode_impl(cotr_model* m, const float* img, int B, cotr_context* ctx, cudaS
     COTR_CHECK(ctx && ctx->model == m, "cotr_encode_context: context does not belong to this model");
     COTR_CHECK(B <= ctx->max_pairs, "cotr_encode_context: B = %d exceeds the context capacity %d", B, ctx->max_pairs);
     COTR_CHECK_CUDA(cudaSetDevice(m->device));
-    if (ensure_encode_ws(m, B) || ensure_sync_ctr(m)) return 1;
+    if (ensure_encode_ws(m, B)) return 1;
     Workspace& w = m->ws;
-    SyncPlan plan;
-    plan.on = dataflow_enabled(m);
-    plan.base = w.sync_ctr;
-    plan.cap_blocks = kSyncEncodeBlocks;
-    if (plan.on) COTR_CHECK_CUDA(cudaMemsetAsync(w.sync_ctr, 0, (size_t)kSyncEncodeBlocks * kSyncBlockInts * sizeof(int), s));
-    Run r{m, s, &plan};
+    Run r{m, s};
     const int n_img = 2 * B;
     const CSplit16 none{nullptr, nullptr};
 
@@ -679,19 +577,12 @@ int encode_impl(cotr_model* m, const float* img, int B, cotr_context* ctx, cudaS
     // Stem: conv 7x7/2 (+FrozenBN folded) + ReLU, then MaxPool 3x3/2  (torchvision resnet.py _forward_impl).
     {
         LaunchScope scope(r, K_STEM_CANVAS, n_img * 256 * 256, 4, 0);
-        LaunchSync y = plan_dep(r, DEP_ALL, n_img * 256 * 256);
-        if (launch_stem_canvas(img, w.canvas, n_img, s, y)) return 1;
-        const size_t blocks = ((size_t)n_img * 256 * 256 + 255) / 256;
-        plan_done(r, y, (int)(blocks < kNumSms * 16 ? blocks : kNumSms * 16), 0, n_img * 256 * 256);
+        if (launch_stem_canvas(img, w.canvas, n_img, s)) return 1;
     }
     if (run_conv(r, m->stem, n_img, cs(w.canvas), 256, 256, w.stem, true, none)) return 1;
     {
         LaunchScope scope(r, K_MAXPOOL, n_img * 64 * 64, 64, 0);
-        LaunchSync y = plan_dep(r, DEP_ALL, n_img * 64 * 64);
-        if (launch_maxpool_3x3s2_nhwc(cs(w.stem), w.bx, n_img, 128, 128, 64, s, y)) return 1;
-        const size_t total = (size_t)n_img * 64 * 64 * 8;
-        const size_t blocks = (total + 255) / 256;
-        plan_done(r, y, (int)(blocks < kNumSms * 16 ? blocks : kNumSms * 16), 0, n_img * 64 * 64);
+        if (launch_maxpool_3x3s2_nhwc(cs(w.stem), w.bx, n_img, 128, 128, 64, s)) return 1;
     }
 
     Split16 x = w.bx;
@@ -731,32 +622,27 @@ int encode_impl(cotr_model* m, const float* img, int B, cotr_context* ctx, cudaS
         // producer writes the pre-norm rows (xa: x + attention, xb: x1 + FFN) and every consumer applies the norm on
         // the fly (GemmParams::a_ln_cs for GEMM inputs, res_ln_part for residual operands) from the partial row
         // statistics the producer's epilogue leaves behind: enc_st_a belongs to xa (norm1), enc_st_b to xb (norm2).
-        const int n_enc_dbg = (g_tc_variant >> 20) & 7;        // bring-up: stop after this many encoder layers (0 = all)
-        for (int l = 0; l < (n_enc_dbg ? n_enc_dbg : kEncLayers); ++l) {
+        for (int l = 0; l < kEncLayers; ++l) {
             const EncLayer& e = m->enc[l];
             const bool ln_in = l > 0;          // the layer input is LN2_{l-1}(xb), deferred
-            // q|k and v^T alternate between two buffers: with tile-level dependencies the next layer's projection of a
-            // row tile may run while other tiles of this layer still attend to the old keys / values
-            const Split16 qk_l = (l & 1) ? w.qk2 : w.qk, vt_l = (l & 1) ? w.vt2 : w.vt;
-            unsigned char* const kvimg_l = (l & 1) ? w.kvimg2 : w.kvimg;
             {
-                GemmParams p = gemm_base(T, 3 * kDModel, kDModel, cs(xin), kDModel, e.qkv.w, e.qkv.wtc, e.qkv.wtc_scale, qk_l, 2 * kDModel);
+                GemmParams p = gemm_base(T, 3 * kDModel, kDModel, cs(xin), kDModel, e.qkv.w, e.qkv.wtc, e.qkv.wtc_scale, w.qk, 2 * kDModel);
                 p.addmat = e.add_qkv_tc; p.add_period = kTokens; p.ld_add = 3 * kDModel;
                 p.remap = 1;
                 p.blk_map[0] = 0; p.blk_map[1] = kDModel; p.blk_map[2] = -1;
-                p.vt = vt_l; p.n_vt = 1;
-                p.kv_img = kvimg_l; p.blk_map[1] = -1000;           // keys and values go straight into the attention operand images
+                p.vt = w.vt; p.n_vt = 1;
+                p.kv_img = w.kvimg; p.blk_map[1] = -1000;           // keys and values go straight into the attention operand images
                 if (ln_in) { p.a_ln_cs = e.qkv.cs; p.a_ln_part = w.enc_st_b; }
-                if (launch_tc(r, p, DEP_TILE)) return 1;
+                if (launch_tc(r, p)) return 1;
             }
             AttnParams a{};
-            a.q = cs(qk_l); a.ldq = 2 * kDModel;
-            a.k = offset(cs(qk_l), kDModel); a.ldk = 2 * kDModel;
-            a.vt = cs(vt_l); a.vt_pair_stride = kVtLayer;
-            a.kv_img = kvimg_l; a.img_pair_stride = kHeads * kAttnHeadImgBytes;
+            a.q = cs(w.qk); a.ldq = 2 * kDModel;
+            a.k = offset(cs(w.qk), kDModel); a.ldk = 2 * kDModel;
+            a.vt = cs(w.vt); a.vt_pair_stride = kVtLayer;
+            a.kv_img = w.kvimg; a.img_pair_stride = kHeads * kAttnHeadImgBytes;
             a.out = w.ao; a.ldo = kDModel;
             a.nq = kTokens; a.npairs = B; a.pair0 = 0;
-            if (run_attention(r, a, DEP_SPAN, kTokens / 128)) return 1;
+            if (run_attention(r, a)) return 1;
             // xa = x + out_proj(attn)                                   (transformer.py:149-154, norm1 deferred)
             if (run_linear_dln(r, e.o, T, cs(w.ao), kDModel, w.xa, kDModel, false, nullptr, w.enc_st_a, cs(xin), kDModel,
                                ln_in ? w.enc_st_b : nullptr, ln_in ? m->enc[l - 1].ln2_g : nullptr, ln_in ? m->enc[l - 1].ln2_b : nullptr)) return 1;
@@ -782,7 +668,7 @@ int encode_impl(cotr_model* m, const float* img, int B, cotr_context* ctx, cudaS
             p.kv_img = ctx->img;
             for (int l = 0; l < kDecLayers; ++l) p.blk_map[2 * l] = -1000 - l;
             p.a_ln_cs = m->kv_all.cs; p.a_ln_part = w.enc_st_b;
-            if (launch_tc(r, p, DEP_TILE)) return 1;
+            if (launch_tc(r, p)) return 1;
         }
         ctx->pairs = B;
         ctx->holds_img = true;
@@ -792,8 +678,7 @@ int encode_impl(cotr_model* m, const float* img, int B, cotr_context* ctx, cudaS
     // default schedule (and the fp32 SIMT cross-check path): explicit LayerNorm launches, the checkpoint's weights as they are
     m->last_mem_pre_ln = false;
     const bool tc = m->gemm_path == 0;      // tensor-core path: keys / values are written as attention operand images
-    const int n_enc_dbg = (g_tc_variant >> 20) & 7;
-    for (int l = 0; l < (n_enc_dbg ? n_enc_dbg : kEncLayers); ++l) {
+    for (int l = 0; l < kEncLayers; ++l) {
         const EncLayer& e = m->enc[l];
         {
             GemmParams p = gemm_base(T, 3 * kDModel, kDModel, cs(xin), kDModel, e.qkv.w, e.qkv.wtc_plain ? e.qkv.wtc_plain : e.qkv.wtc, e.qkv.wtc_plain ? e.qkv.wtc_plain_scale : e.qkv.wtc_scale, w.qk, 2 * kDModel);
@@ -845,28 +730,19 @@ int encode_impl(cotr_model* m, const float* img, int B, cotr_context* ctx, cudaS
 }
 
 int decode_chunk(cotr_model* m, const cotr_context* ctx, const float* queries, float* pred, int pair0, int npairs,
-                 int nq, cudaStream_t s, int chunk_index) {
+                 int nq, cudaStream_t s) {
     Workspace& w = m->ws;
-    // dataflow counters of this chunk (zeroed by decode_impl); the chunk's first launch has no announced producer and
-    // falls back to the hardware wait, which also orders it behind the previous chunk / the encoder
-    SyncPlan plan;
-    plan.on = dataflow_enabled(m) && kSyncEncodeBlocks + (chunk_index + 1) * kSyncChunkBlocks <= kSyncBlocks;
-    plan.base = w.sync_ctr + (size_t)(kSyncEncodeBlocks + chunk_index * kSyncChunkBlocks) * kSyncBlockInts;
-    plan.cap_blocks = kSyncChunkBlocks;
-    Run r{m, s, &plan};
+    Run r{m, s};
     const int R = npairs * nq;
     const CSplit16 none{nullptr, nullptr};
     // cotr_model.py:34-35 query_proj (lin_sine, depth 64)
     {
         LaunchScope scope(r, K_QENC, R, kDModel, 0);
-        LaunchSync y = plan_dep(r, DEP_ALL, R);
-        y.sig_tiles = (y.sig && (R % 128) == 0) ? sync_tiles_for(R) : 0;      // one block per row: whole tiles only
-        if (launch_query_encode(queries, w.qpos, R, s, y)) return 1;
-        plan_done(r, y, R, 128, R);
+        if (launch_query_encode(queries, w.qpos, R, s)) return 1;
     }
     // q-side of transformer.py:192: ((t + qpos) Wq^T + bq) s  =  t (s Wq)^T + [qpos (s Wq)^T + s bq]; the bracket for
     // all 6 layers is one GEMM.
-    if (run_linear(r, m->qpos_all, R, cs(w.qpos), kDModel, w.qp, kQpCols, false, none, 0, nullptr, nullptr, nullptr, DEP_TILE)) return 1;
+    if (run_linear(r, m->qpos_all, R, cs(w.qpos), kDModel, w.qp, kQpCols, false)) return 1;
 
     if (deferred_ln_enabled(m, R)) {
         // Tensor-core path with deferred LayerNorms (see encode_impl): w.t = t + attention (norm2 deferred),
@@ -888,7 +764,7 @@ int decode_chunk(cotr_model* m, const cotr_context* ctx, const float* queries, f
             if (ctx->holds_img) { a.kv_img = ctx->img + (size_t)l * kHeads * kAttnHeadImgBytes; a.img_pair_stride = (size_t)kDecLayers * kHeads * kAttnHeadImgBytes; }
             a.out = w.dao; a.ldo = kDModel;
             a.nq = nq; a.npairs = npairs; a.pair0 = pair0;
-            if (run_attention(r, a, DEP_TILE)) return 1;
+            if (run_attention(r, a)) return 1;
             // transformer.py:196-197: t = t + out_proj(attn)   (norm2 deferred; t = norm3_{l-1}(t2), deferred, or 0)
             if (run_linear_dln(r, d.o, R, cs(w.dao), kDModel, w.t, kDModel, false, nullptr, w.dec_st_a, ln_in ? cs(w.t2) : none, kDModel,
                                ln_in ? w.dec_st_b : nullptr, ln_in ? m->dec[l - 1].ln3_g : nullptr, ln_in ? m->dec[l - 1].ln3_b : nullptr)) return 1;
@@ -901,10 +777,7 @@ int decode_chunk(cotr_model* m, const cotr_context* ctx, const float* queries, f
         {
             const DecLayer& d = m->dec[kDecLayers - 1];
             LaunchScope scope(r, K_LAYERNORM, R, kDModel, 0);
-            LaunchSync y = plan_dep(r, DEP_TILE, R);
-            y.sig_tiles = (y.sig && (R % 128) == 0) ? sync_tiles_for(R) : 0;      // 8 rows per block: whole tiles only
-            if (launch_layernorm_twice(cs(w.t2), d.ln3_g, d.ln3_b, m->dec_norm_g, m->dec_norm_b, w.hs, R, s, y)) return 1;
-            plan_done(r, y, (R + 7) / 8, 16, R);
+            if (launch_layernorm_twice(cs(w.t2), d.ln3_g, d.ln3_b, m->dec_norm_g, m->dec_norm_b, w.hs, R, s)) return 1;
         }
     } else {
         for (int l = 0; l < kDecLayers; ++l) {
@@ -935,13 +808,13 @@ int decode_chunk(cotr_model* m, const cotr_context* ctx, const float* queries, f
             if (launch_layernorm(cs(w.t), m->dec_norm_g, m->dec_norm_b, w.hs, R, s)) return 1;
         }
     }
-    if (run_linear(r, m->head[0], R, cs(w.hs), kDModel, w.hd1, kDModel, true, none, 0, nullptr, nullptr, nullptr, DEP_TILE)) return 1;
-    if (run_linear(r, m->head[1], R, cs(w.hd1), kDModel, w.hd2, kDModel, true, none, 0, nullptr, nullptr, nullptr, DEP_TILE)) return 1;
+    if (run_linear(r, m->head[0], R, cs(w.hs), kDModel, w.hd1, kDModel, true)) return 1;
+    if (run_linear(r, m->head[1], R, cs(w.hd1), kDModel, w.hd2, kDModel, true)) return 1;
     {
         GemmParams p = gemm_base(R, 2, kDModel, cs(w.hd2), kDModel, m->head[2].w, m->head[2].wtc, m->head[2].wtc_scale, kNoSplit, 2);
         p.bias = m->head[2].b;
         p.out_f32 = pred;
-        if (run_gemm(r, p, nullptr, DEP_TILE)) return 1;
+        if (run_gemm(r, p, nullptr)) return 1;
     }
     return 0;
 }
@@ -956,32 +829,19 @@ int decode_impl(cotr_model* m, const cotr_context* ctx, const float* queries, in
     COTR_CHECK_CUDA(cudaSetDevice(m->device));
     const long long total = (long long)B * Q;
     const int cap = (int)(total < kDecodeChunkRows ? total : kDecodeChunkRows);
-    if (ensure_decode_ws(m, cap) || ensure_sync_ctr(m)) return 1;
-    int n_chunks = 0;
-    if (Q <= kDecodeChunkRows) {
-        const int pairs_per = kDecodeChunkRows / Q;
-        n_chunks = (B + pairs_per - 1) / pairs_per;
-    } else {
-        n_chunks = B * ((Q + kDecodeChunkRows - 1) / kDecodeChunkRows);
-    }
-    if (dataflow_enabled(m)) {
-        const int blocks = std::min(kSyncBlocks - kSyncEncodeBlocks, n_chunks * kSyncChunkBlocks);
-        COTR_CHECK_CUDA(cudaMemsetAsync(m->ws.sync_ctr + (size_t)kSyncEncodeBlocks * kSyncBlockInts, 0,
-                                        (size_t)blocks * kSyncBlockInts * sizeof(int), s));
-    }
-    int chunk = 0;
+    if (ensure_decode_ws(m, cap)) return 1;
     if (Q <= kDecodeChunkRows) {
         const int pairs_per = kDecodeChunkRows / Q;
         for (int b0 = 0; b0 < B; b0 += pairs_per) {
             const int nb = (B - b0 < pairs_per) ? B - b0 : pairs_per;
-            if (decode_chunk(m, ctx, queries + (size_t)b0 * Q * 2, pred + (size_t)b0 * Q * 2, b0, nb, Q, s, chunk++)) return 1;
+            if (decode_chunk(m, ctx, queries + (size_t)b0 * Q * 2, pred + (size_t)b0 * Q * 2, b0, nb, Q, s)) return 1;
         }
     } else {
         for (int b = 0; b < B; ++b)
             for (int q0 = 0; q0 < Q; q0 += kDecodeChunkRows) {
                 const int nq = (Q - q0 < kDecodeChunkRows) ? Q - q0 : kDecodeChunkRows;
                 const size_t off = ((size_t)b * Q + q0) * 2;
-                if (decode_chunk(m, ctx, queries + off, pred + off, b, 1, nq, s, chunk++)) return 1;
+                if (decode_chunk(m, ctx, queries + off, pred + off, b, 1, nq, s)) return 1;
             }
     }
     m->last_rows = (total <= kDecodeChunkRows) ? (int)total : 0;
@@ -1206,11 +1066,9 @@ void cotr_destroy(cotr_model* m) {
     for (void* p : m->allocs) cudaFree(p);
     Workspace& w = m->ws;
     Split16* bufs[] = {&w.canvas, &w.stem, &w.bx, &w.by, &w.bt1, &w.bt2, &w.bds, &w.src, &w.xa, &w.xb, &w.qk, &w.vt, &w.ao, &w.ffh,
-                       &w.qpos, &w.qp, &w.t, &w.qb, &w.dao, &w.dh, &w.hs, &w.hd1, &w.hd2, &w.t2, &w.qk2, &w.vt2};
+                       &w.qpos, &w.qp, &w.t, &w.qb, &w.dao, &w.dh, &w.hs, &w.hd1, &w.hd2, &w.t2};
     for (Split16* b : bufs) ws_free(b);
-    if (w.sync_ctr) cudaFree(w.sync_ctr);
     if (w.kvimg) cudaFree(w.kvimg);
-    if (w.kvimg2) cudaFree(w.kvimg2);
     float** fbufs[] = {&w.ln_tmp, &w.dln_tmp, &w.img_stage, &w.q_stage, &w.pred_stage,
                        reinterpret_cast<float**>(&w.enc_st_a), reinterpret_cast<float**>(&w.enc_st_b),
                        reinterpret_cast<float**>(&w.dec_st_a), reinterpret_cast<float**>(&w.dec_st_b)};
@@ -1304,7 +1162,7 @@ int forward_eager(cotr_model* m, const float* img, const float* queries, int B, 
 // Forward on the staging buffers (img_stage, q_stage -> pred_stage): graph replay when a graph exists for the shape.
 int forward_staged(cotr_model* m, int B, int Q, cudaStream_t s) {
     Workspace& w = m->ws;
-    const bool graphable = m->graph_mode && !m->prof_on && (g_tc_timestamps == nullptr || (g_tc_variant & (1 << 17)));
+    const bool graphable = m->graph_mode && !m->prof_on;
     const long long key = ((long long)B << 32) | (unsigned)Q;
     if (graphable) {
         auto it = m->graphs.find(key);
@@ -1349,7 +1207,7 @@ int cotr_forward(cotr_model* m, const float* img_dev, const float* queries_dev, 
     COTR_CHECK_CUDA(cudaSetDevice(m->device));
     cudaStream_t s = (cudaStream_t)cuda_stream;
     CallOrder order(m, s);
-    const bool graphable = m->graph_mode && !m->prof_on && (g_tc_timestamps == nullptr || (g_tc_variant & (1 << 17))) && Q > 0;
+    const bool graphable = m->graph_mode && !m->prof_on && Q > 0;
     if (!graphable) return forward_eager(m, img_dev, queries_dev, B, Q, pred_dev, s);
     // graph replay needs fixed addresses: go through the staging buffers (two small device-to-device copies in, one out)
     if (ensure_stage(m, B, Q)) return 1;
@@ -1523,10 +1381,6 @@ int cotr_set_gemm_path(cotr_model* m, int path) {
 }
 
 void cotr_debug_set_variant(int variant) { g_tc_variant = variant; g_use_pdl = (variant & 256) ? 0 : 1; }
-void cotr_debug_set_timestamps(void* dev_buffer) {
-    g_tc_timestamps = reinterpret_cast<long long*>(dev_buffer);
-    g_tc_trace_idx = 0;
-}
 
 // ---- kernel-level test hooks: fp32 device tensors in / out, converted to split16 around the kernel under test -------
 namespace {

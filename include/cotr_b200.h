@@ -218,18 +218,11 @@ int cotr_test_attention(int path, const float* q_dev, const float* k_dev, const 
                         int nq, int npairs);
 /* bring-up / A-B switches (0 = production): bit 8 (256) disables programmatic dependent launch, bit 9 (512) disables
  * split-K, bits 10-11 move the CTA-count threshold of the 64-wide GEMM tile, bits 14-15 lower the
- * minimum K of split-K (16 >> n chunks of 64), bit 17 selects trace mode for cotr_debug_set_timestamps, bits 20-22 stop
- * the encoder after n layers.  Schedule: by default a transformer section with >= 2048 rows runs the deferred-LayerNorm
- * schedule (no LayerNorm launches), smaller ones the explicit one; bit 19 forces deferred everywhere, bit 16 never;
- * bits 19 + 18 add the counter-based dataflow dependencies (experimental).
+ * minimum K of split-K (16 >> n chunks of 64).  Schedule: by default a transformer section with >= 2048 rows runs the
+ * deferred-LayerNorm schedule (no LayerNorm launches), smaller ones the explicit one; bit 19 forces deferred
+ * everywhere, bit 16 never.
  * Process-wide; graphs captured under another value are NOT dropped (call cotr_set_gemm_path twice to drop them). */
 void cotr_debug_set_variant(int variant);
-/* debug timeline of the tensor-core kernels: DEVICE buffer of 64 int64 per CTA receiving clock64() deltas of the pipeline
- * events of every following GEMM / attention launch (NULL switches it off; graph replay is off while it is set).
- * Slot layout: the COTR_TS marks in gemm_tc.cu / attention_tc.cu.  Trace mode (variant bit 17): the buffer holds
- * 256 x 64 slots PER LAUNCH (launch counter reset by this call), slot 62 receives %globaltimer at CTA exit, and graph
- * replay stays on, so a per-launch schedule of one forward can be reconstructed from it. */
-void cotr_debug_set_timestamps(void* dev_buffer);
 
 const char* cotr_last_error(void);
 const char* cotr_version(void);

@@ -182,13 +182,11 @@ def test_graph_replay_survives_workspace_growth(built_lib):
     torch.cuda.synchronize()
 
 
-@pytest.mark.parametrize("variant,name", [(1 << 19, "deferred-layernorm"), ((1 << 19) | (1 << 18), "deferred-layernorm+dataflow"),
-                                          (1 << 16, "explicit-layernorm")])
+@pytest.mark.parametrize("variant,name", [(1 << 19, "deferred-layernorm"), (1 << 16, "explicit-layernorm")])
 def test_experimental_schedules_match_the_reference(golden_dir, built_lib, variant, name):
     """The schedules cotr_debug_set_variant can force (bit 19: LayerNorms applied on the fly by their consumers from
-    partial row statistics, everywhere; bits 19 + 18: launch-to-launch dependencies through counters in global memory
-    instead of griddepcontrol.wait; bit 16: explicit LayerNorm launches everywhere - by default each section picks by
-    its row count) all stay correct: same goldens, same tolerance, eager and
+    partial row statistics, everywhere; bit 16: explicit LayerNorm launches everywhere - by default each section picks
+    by its row count) both stay correct: same goldens, same tolerance, eager and
     graph-replayed, also for a batch whose query count is not a tile multiple."""
     from cotr_b200 import capi
     capi.lib().cotr_debug_set_variant(variant)
