@@ -66,7 +66,7 @@ inline cudaError_t launch_kernel(void (*kernel)(KArgs...), dim3 grid, dim3 block
     return cudaLaunchKernelEx(&cfg, kernel, KArgs(args)...);
 }
 
-// Same, with a thread-block cluster of (1, 1, cluster_z) CTAs (grid.z must equal cluster_z).
+// Same, with a thread-block cluster of (1, 1, cluster_z) CTAs (grid.z must be a multiple of cluster_z).
 template <typename... KArgs, typename... Args>
 inline cudaError_t launch_kernel_cluster(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t s,
                                          int cluster_z, Args... args) {
@@ -107,7 +107,8 @@ constexpr int kDecLayers = 6;
 
 // Attention operand images (tensor-core path).  The keys and values of one (pair, slot, head) - slot = decoder layer, or 0
 // for the encoder's own layer - are stored in HBM exactly as the attention kernel wants them in shared memory, so that
-// staging them is two bulk-TMA copies issued by one thread (cp.async.bulk -> UBLKCP) instead of 8 192 16-byte cp.async:
+// staging them is two bulk-TMA copies issued by one thread (cp.async.bulk -> UBLKCP) instead of 8 192 16-byte cp.async
+// (a CTA that owns a slice of the keys copies 8 runs of K and one of V):
 //   K image  [plane hi | lo][4 groups of 8 head dims][512 keys][16 B]           = 2 x 32 KB  (wgmma K-major canonical layout)
 //   V image  [64 groups of 8 keys][hi: 32 head dims x 16 B | lo: 32 x 16 B | 16 B pad]  = 64 x 1040 B
 // written in that form by the epilogue of the projection GEMM (split16.cuh::store16).
