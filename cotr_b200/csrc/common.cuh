@@ -226,7 +226,24 @@ struct AttnParams {
     int pair0;
 };
 
+// A transformer feed-forward block with its residual and post-LayerNorm (mlp_tc.cu):
+//   out = LN(x + W2 relu(W1 x + b1) + b2), then optionally a second LayerNorm (g2 / be2);  x, out: [M][256], may alias.
+struct MlpParams {
+    int M;
+    CSplit16 x;
+    Split16 out;
+    const void* w1;      // tensor-core image of linear1 [1024][256] (gemm_tc.cu tc_pack_weight)
+    float w1_scale;
+    const float* b1;
+    const void* w2;      // tensor-core image of linear2 [256][1024]
+    float w2_scale;
+    const float* b2;
+    const float *g, *be;
+    const float *g2, *be2;     // null: no second LayerNorm
+};
+
 int launch_gemm_simt(const GemmParams& p, cudaStream_t s);
+int launch_mlp_tc(const MlpParams& p, cudaStream_t s);
 int launch_gemm_simt_raw(const GemmParams& p, float* raw_out_f32, cudaStream_t s);   // result as plain fp32 [M,N]
 int launch_layernorm_f32(const float* x, const float* gamma, const float* beta, Split16 out, int rows, cudaStream_t s);
 int launch_gemm_tc(const GemmParams& p, cudaStream_t s);

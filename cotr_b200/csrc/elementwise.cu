@@ -59,35 +59,6 @@ __global__ void __launch_bounds__(256) stem_canvas_kernel(const float* __restric
     }
 }
 
-__device__ __forceinline__ float warp_sum(float v) {
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-    return v;
-}
-
-// out = LayerNorm(x) over 256 channels, eps 1e-5, biased variance.  One warp per row, 8 channels per lane.
-__device__ __forceinline__ void load_vec8(const float* __restrict__ p, int lane, float (&v)[8]) {
-    const float4 a = __ldg(reinterpret_cast<const float4*>(p + lane * 8)), b = __ldg(reinterpret_cast<const float4*>(p + lane * 8 + 4));
-    v[0] = a.x; v[1] = a.y; v[2] = a.z; v[3] = a.w; v[4] = b.x; v[5] = b.y; v[6] = b.z; v[7] = b.w;
-}
-
-// v (8 channels per lane of one warp) <- LayerNorm over the 256 channels of the row
-__device__ __forceinline__ void warp_layernorm256(float (&v)[8], const float* __restrict__ gamma, const float* __restrict__ beta, int lane) {
-    float s = 0.f;
-#pragma unroll
-    for (int j = 0; j < 8; ++j) s += v[j];
-    const float mean = warp_sum(s) * (1.f / kDModel);
-    float sq = 0.f;
-#pragma unroll
-    for (int j = 0; j < 8; ++j) { v[j] -= mean; sq = fmaf(v[j], v[j], sq); }
-    const float rstd = 1.f / sqrtf(warp_sum(sq) * (1.f / kDModel) + 1e-5f);
-    float g[8], b[8];
-    load_vec8(gamma, lane, g);
-    load_vec8(beta, lane, b);
-#pragma unroll
-    for (int j = 0; j < 8; ++j) v[j] = v[j] * rstd * g[j] + b[j];
-}
-
 // (mean, M2) of every 16-channel chunk of a row: two neighbouring lanes (8 channels each) share a chunk
 __global__ void __launch_bounds__(256) ln_partials_kernel(const CSplit16 x, float2* __restrict__ part, int rows) {
     const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;

@@ -309,7 +309,8 @@ struct Run {
     cudaStream_t s;
 };
 
-enum KernelId { K_GEMM_TC = 0, K_GEMM_SIMT = 1, K_ATTN_TC = 2, K_ATTN_SIMT = 3, K_LAYERNORM = 4, K_MAXPOOL = 5, K_QENC = 6, K_STEM_CANVAS = 7 };
+enum KernelId { K_GEMM_TC = 0, K_GEMM_SIMT = 1, K_ATTN_TC = 2, K_ATTN_SIMT = 3, K_LAYERNORM = 4, K_MAXPOOL = 5, K_QENC = 6, K_STEM_CANVAS = 7,
+                K_GEMM_MLP = 8 };
 
 // Counts the launch and, when the profiler is on, brackets it with two events on the launching stream.
 struct LaunchScope {
@@ -399,6 +400,20 @@ int run_linear(const Run& r, const DevLinear& L, int M, CSplit16 A, int lda, Spl
     return run_gemm(r, p, ln_scratch);
 }
 
+// Tensor-core path only: out = LN(x + linear2(relu(linear1(x)))) [-> LN(g2, b2)] in one launch (mlp_tc.cu).  Recorded as
+// M = rows, N = 1024, K = 512, so that 2 M N K is the FLOP count of both GEMMs.
+int run_mlp(const Run& r, const DevLinear& l1, const DevLinear& l2, int M, CSplit16 x, Split16 out, const float* g, const float* b,
+            const float* g2 = nullptr, const float* b2 = nullptr) {
+    MlpParams p;
+    memset(&p, 0, sizeof(p));
+    p.M = M; p.x = x; p.out = out;
+    p.w1 = l1.wtc_plain ? l1.wtc_plain : l1.wtc; p.w1_scale = l1.wtc_plain ? l1.wtc_plain_scale : l1.wtc_scale; p.b1 = l1.b;
+    p.w2 = l2.wtc_plain ? l2.wtc_plain : l2.wtc; p.w2_scale = l2.wtc_plain ? l2.wtc_plain_scale : l2.wtc_scale; p.b2 = l2.b;
+    p.g = g; p.be = b; p.g2 = g2; p.be2 = b2;
+    LaunchScope scope(r, K_GEMM_MLP, M, kFF, 2 * kDModel);
+    return launch_mlp_tc(p, r.s);
+}
+
 // Tensor-core path only: linear layer with deferred LayerNorms (GemmParams::a_ln_cs / res_ln_part / ln_part_out).
 //   a_part     non-null: A holds pre-LayerNorm rows with these partial statistics; L was built by make_linear_ln
 //   part_out   non-null: the output rows are pre-LayerNorm rows of a later norm - leave their partial statistics here
@@ -484,6 +499,11 @@ constexpr int kDeferredLnMinRows = 2048;
 inline bool deferred_ln_enabled(const cotr_model* m, int rows) {
     if (m->gemm_path != 0 || (g_tc_variant & (1 << 16))) return false;
     return (g_tc_variant & (1 << 19)) != 0 || rows >= kDeferredLnMinRows;
+}
+// In the explicit-LayerNorm schedule on the tensor-core path each feed-forward block (linear1, linear2, norm) is one
+// fused launch (run_mlp); bit 16 keeps the separate launches.
+inline bool fused_mlp_enabled(const cotr_model* m) {
+    return m->gemm_path == 0 && !(g_tc_variant & (1 << 16));
 }
 
 // Captured graphs embed workspace / staging / context addresses: whenever one of those is reallocated every graph is
@@ -678,6 +698,7 @@ int encode_impl(cotr_model* m, const float* img, int B, cotr_context* ctx, cudaS
     // default schedule (and the fp32 SIMT cross-check path): explicit LayerNorm launches, the checkpoint's weights as they are
     m->last_mem_pre_ln = false;
     const bool tc = m->gemm_path == 0;      // tensor-core path: keys / values are written as attention operand images
+    const bool fused_mlp = fused_mlp_enabled(m);
     for (int l = 0; l < kEncLayers; ++l) {
         const EncLayer& e = m->enc[l];
         {
@@ -700,8 +721,12 @@ int encode_impl(cotr_model* m, const float* img, int B, cotr_context* ctx, cudaS
         // x1 = LN1(x + out_proj(attn))
         if (run_linear(r, e.o, T, cs(w.ao), kDModel, w.xa, kDModel, false, cs(xin), kDModel, e.ln1_g, e.ln1_b, w.ln_tmp)) return 1;
         // x2 = LN2(x1 + W2 relu(W1 x1 + b1) + b2)
-        if (run_linear(r, e.l1, T, cs(w.xa), kDModel, w.ffh, kFF, true)) return 1;
-        if (run_linear(r, e.l2, T, cs(w.ffh), kFF, w.xb, kDModel, false, cs(w.xa), kDModel, e.ln2_g, e.ln2_b, w.ln_tmp)) return 1;
+        if (fused_mlp) {
+            if (run_mlp(r, e.l1, e.l2, T, cs(w.xa), w.xb, e.ln2_g, e.ln2_b)) return 1;
+        } else {
+            if (run_linear(r, e.l1, T, cs(w.xa), kDModel, w.ffh, kFF, true)) return 1;
+            if (run_linear(r, e.l2, T, cs(w.ffh), kFF, w.xb, kDModel, false, cs(w.xa), kDModel, e.ln2_g, e.ln2_b, w.ln_tmp)) return 1;
+        }
         xin = w.xb;
     }
     m->last_mem = xin;
@@ -780,6 +805,7 @@ int decode_chunk(cotr_model* m, const cotr_context* ctx, const float* queries, f
             if (launch_layernorm_twice(cs(w.t2), d.ln3_g, d.ln3_b, m->dec_norm_g, m->dec_norm_b, w.hs, R, s)) return 1;
         }
     } else {
+        const bool fused_mlp = fused_mlp_enabled(m);
         for (int l = 0; l < kDecLayers; ++l) {
             const DecLayer& d = m->dec[l];
             CSplit16 q = cs(w.qp);      // layer 0: tgt = 0 (transformer.py:54), so q is the qpos projection alone
@@ -799,11 +825,18 @@ int decode_chunk(cotr_model* m, const cotr_context* ctx, const float* queries, f
             // transformer.py:196-197: t = norm2(t + out_proj(attn))
             if (run_linear(r, d.o, R, cs(w.dao), kDModel, w.t, kDModel, false, l > 0 ? cs(w.t) : none, kDModel, d.ln2_g, d.ln2_b, w.dln_tmp)) return 1;
             // transformer.py:198-200: t = norm3(t + linear2(relu(linear1(t))))
-            if (run_linear(r, d.l1, R, cs(w.t), kDModel, w.dh, kFF, true)) return 1;
-            if (run_linear(r, d.l2, R, cs(w.dh), kFF, w.t, kDModel, false, cs(w.t), kDModel, d.ln3_g, d.ln3_b, w.dln_tmp)) return 1;
+            if (fused_mlp) {
+                // in place; the last layer also applies transformer.py:110-111 decoder.norm and writes hs
+                const bool last = l == kDecLayers - 1;
+                if (run_mlp(r, d.l1, d.l2, R, cs(w.t), last ? w.hs : w.t, d.ln3_g, d.ln3_b,
+                            last ? m->dec_norm_g : nullptr, last ? m->dec_norm_b : nullptr)) return 1;
+            } else {
+                if (run_linear(r, d.l1, R, cs(w.t), kDModel, w.dh, kFF, true)) return 1;
+                if (run_linear(r, d.l2, R, cs(w.dh), kFF, w.t, kDModel, false, cs(w.t), kDModel, d.ln3_g, d.ln3_b, w.dln_tmp)) return 1;
+            }
         }
         // transformer.py:110-111 decoder.norm on the last level; cotr_model.py:38-39 corr_embed on that level only.
-        {
+        if (!fused_mlp) {
             LaunchScope scope(r, K_LAYERNORM, R, kDModel, 0);
             if (launch_layernorm(cs(w.t), m->dec_norm_g, m->dec_norm_b, w.hs, R, s)) return 1;
         }

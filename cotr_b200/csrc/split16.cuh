@@ -54,6 +54,35 @@ __device__ __forceinline__ void store8_split(const Split16& t, size_t off, const
     *reinterpret_cast<uint4*>(t.lo + off) = l;
 }
 
+__device__ __forceinline__ float warp_sum(float v) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+    return v;
+}
+
+// out = LayerNorm(x) over 256 channels, eps 1e-5, biased variance.  One warp per row, 8 channels per lane.
+__device__ __forceinline__ void load_vec8(const float* __restrict__ p, int lane, float (&v)[8]) {
+    const float4 a = __ldg(reinterpret_cast<const float4*>(p + lane * 8)), b = __ldg(reinterpret_cast<const float4*>(p + lane * 8 + 4));
+    v[0] = a.x; v[1] = a.y; v[2] = a.z; v[3] = a.w; v[4] = b.x; v[5] = b.y; v[6] = b.z; v[7] = b.w;
+}
+
+// v (8 channels per lane of one warp) <- LayerNorm over the 256 channels of the row
+__device__ __forceinline__ void warp_layernorm256(float (&v)[8], const float* __restrict__ gamma, const float* __restrict__ beta, int lane) {
+    float s = 0.f;
+#pragma unroll
+    for (int j = 0; j < 8; ++j) s += v[j];
+    const float mean = warp_sum(s) * (1.f / kDModel);
+    float sq = 0.f;
+#pragma unroll
+    for (int j = 0; j < 8; ++j) { v[j] -= mean; sq = fmaf(v[j], v[j], sq); }
+    const float rstd = 1.f / sqrtf(warp_sum(sq) * (1.f / kDModel) + 1e-5f);
+    float g[8], b[8];
+    load_vec8(gamma, lane, g);
+    load_vec8(beta, lane, b);
+#pragma unroll
+    for (int j = 0; j < 8; ++j) v[j] = v[j] * rstd * g[j] + b[j];
+}
+
 // Where column block [nb, nb+16) of output row `row` goes (GemmParams::remap / blk_map): returns true when the
 // block is a transposed value projection, in which case `base` is the vt element offset of (column nb, this row)
 // and consecutive columns are 512 elements apart; otherwise `base` is the row-major element offset.

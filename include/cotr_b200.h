@@ -219,8 +219,9 @@ int cotr_test_attention(int path, const float* q_dev, const float* k_dev, const 
 /* bring-up / A-B switches (0 = production): bit 8 (256) disables programmatic dependent launch, bit 9 (512) disables
  * split-K, bits 10-11 move the CTA-count threshold of the 64-wide GEMM tile, bits 14-15 lower the
  * minimum K of split-K (16 >> n chunks of 64).  Schedule: by default a transformer section with >= 2048 rows runs the
- * deferred-LayerNorm schedule (no LayerNorm launches), smaller ones the explicit one; bit 19 forces deferred
- * everywhere, bit 16 never.
+ * deferred-LayerNorm schedule (no LayerNorm launches), smaller ones the explicit one, in which each feed-forward block
+ * (linear1, linear2, its LayerNorm) is one fused launch on the tensor-core path; bit 19 forces deferred everywhere,
+ * bit 16 never and runs every feed-forward block as separate linear1 / linear2 / LayerNorm launches.
  * Process-wide; graphs captured under another value are NOT dropped (call cotr_set_gemm_path twice to drop them). */
 void cotr_debug_set_variant(int variant);
 
