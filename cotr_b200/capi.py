@@ -30,7 +30,8 @@ class LaunchRecord(ctypes.Structure):
                 ("ms", ctypes.c_float)]
 
 
-KERNEL_NAMES = ("gemm_tc", "gemm_simt", "attention_tc", "attention_simt", "layernorm", "maxpool", "query_encode", "stem_canvas", "gemm_mlp")
+KERNEL_NAMES = ("gemm_tc", "gemm_simt", "attention_tc", "attention_simt", "layernorm", "maxpool", "query_encode", "stem_canvas", "gemm_mlp",
+                "attention_weights_tc", "attention_weights_simt")
 
 # name -> (restype, argtypes); every symbol include/cotr_b200.h declares
 _PROTOTYPES = {
@@ -40,6 +41,10 @@ _PROTOTYPES = {
     "cotr_context_destroy": (None, [ctypes.c_void_p]),
     "cotr_encode_context": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p]),
     "cotr_decode": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p]),
+    "cotr_encode_context_attention": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p, ctypes.c_int,
+                                                     ctypes.c_void_p, ctypes.c_void_p]),
+    "cotr_decode_attention": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int,
+                                             ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]),
     "cotr_forward": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p]),
     "cotr_forward_host": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_void_p]),
     "cotr_preprocess": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_void_p, ctypes.c_int,
@@ -67,6 +72,7 @@ _PROTOTYPES = {
     "cotr_set_gemm_path": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_int]),
     "cotr_test_gemm": (ctypes.c_int, [ctypes.POINTER(TestGemmDesc)] + [ctypes.c_void_p] * 9),
     "cotr_test_attention": (ctypes.c_int, [ctypes.c_int] + [ctypes.c_void_p] * 4 + [ctypes.c_int, ctypes.c_int]),
+    "cotr_test_attention_weights": (ctypes.c_int, [ctypes.c_int] + [ctypes.c_void_p] * 3 + [ctypes.c_int, ctypes.c_int]),
     "cotr_debug_set_variant": (None, [ctypes.c_int]),
     "cotr_last_error": (ctypes.c_char_p, []),
     "cotr_version": (ctypes.c_char_p, []),
@@ -177,6 +183,26 @@ class NativeModel:
         pred = torch.empty((B, Q, 2), dtype=torch.float32, device=queries.device)
         check(lib().cotr_decode(self.handle, ctx.handle, _ptr(queries), B, Q, _ptr(pred), self._stream()), "cotr_decode")
         return pred
+
+    def encode_context_attention(self, img, ctx, layer_mask):
+        """encode_context that also returns the head-averaged attention maps of the encoder layers selected by
+        `layer_mask` (bit l = layer l): (popcount(layer_mask), B, 512, 512) fp32 (cotr_encode_context_attention)."""
+        B = img.shape[0]
+        attn = torch.empty((bin(layer_mask).count("1"), B, 512, 512), dtype=torch.float32, device=img.device)
+        check(lib().cotr_encode_context_attention(self.handle, _ptr(img), B, ctx.handle, int(layer_mask),
+                                                  _ptr(attn) if layer_mask else None, self._stream()), "cotr_encode_context_attention")
+        ctx.pairs = B
+        return attn
+
+    def decode_attention(self, ctx, queries, layer_mask):
+        """decode that also returns the head-averaged attention maps of the decoder layers selected by `layer_mask`:
+        -> (pred (B,Q,2), maps (popcount(layer_mask), B, Q, 512) fp32) (cotr_decode_attention)."""
+        B, Q = queries.shape[0], queries.shape[1]
+        pred = torch.empty((B, Q, 2), dtype=torch.float32, device=queries.device)
+        attn = torch.empty((bin(layer_mask).count("1"), B, Q, 512), dtype=torch.float32, device=queries.device)
+        check(lib().cotr_decode_attention(self.handle, ctx.handle, _ptr(queries), B, Q, int(layer_mask),
+                                          _ptr(attn) if layer_mask else None, _ptr(pred), self._stream()), "cotr_decode_attention")
+        return pred, attn
 
     def forward_host(self, img_np, queries_np, out_np=None):
         """Host buffers in, host buffer out (H2D + forward + D2H inside the C call)."""
@@ -380,6 +406,13 @@ def test_gemm(path, A, w_host, *, bias=None, addmat=None, add_period=1, residual
     p = lambda t: ctypes.c_void_p(t.data_ptr()) if t is not None else None
     check(lib().cotr_test_gemm(ctypes.byref(d), p(A), ctypes.c_void_p(w_np.ctypes.data), p(bias), p(addmat), p(residual),
                                p(ln[0]) if ln else None, p(ln[1]) if ln else None, p(out), p(part_out)), "cotr_test_gemm")
+    return out
+
+
+def test_attention_weights(path, q, k, nq, npairs):
+    """Kernel-level hook: head-averaged softmax(q k^T) -> (npairs, nq, 512) (cotr_test_attention_weights)."""
+    out = torch.zeros((npairs, nq, 512), dtype=torch.float32, device=q.device)
+    check(lib().cotr_test_attention_weights(path, _ptr(q), _ptr(k), _ptr(out), nq, npairs), "cotr_test_attention_weights")
     return out
 
 

@@ -226,6 +226,21 @@ struct AttnParams {
     int pair0;
 };
 
+// Head-averaged attention weights (attention_weights.cu): out[pair_local][i][key] = (1/8) sum_h softmax(q_h k_h^T)[i][key],
+// the map nn.MultiheadAttention returns with need_weights.  q / k / kv_img / nq / npairs / pair0 as in AttnParams: the
+// tensor-core kernel reads the keys from the operand images, the fp32 SIMT one from the row-major k.
+struct AttnWeightsParams {
+    CSplit16 q; int ldq;
+    CSplit16 k; int ldk;
+    const unsigned char* kv_img;
+    size_t img_pair_stride;
+    float* out;                  // fp32, row i of local pair p at out + p * out_pair_stride + i * 512
+    size_t out_pair_stride;
+    int nq;
+    int npairs;
+    int pair0;
+};
+
 // A transformer feed-forward block with its residual and post-LayerNorm (mlp_tc.cu):
 //   out = LN(x + W2 relu(W1 x + b1) + b2), then optionally a second LayerNorm (g2 / be2);  x, out: [M][256], may alias.
 struct MlpParams {
@@ -249,6 +264,8 @@ int launch_layernorm_f32(const float* x, const float* gamma, const float* beta, 
 int launch_gemm_tc(const GemmParams& p, cudaStream_t s);
 int launch_attention_simt(const AttnParams& p, cudaStream_t s);
 int launch_attention_tc(const AttnParams& p, cudaStream_t s);
+int launch_attention_weights_tc(const AttnWeightsParams& p, cudaStream_t s);
+int launch_attention_weights_simt(const AttnWeightsParams& p, cudaStream_t s);
 int launch_maxpool_3x3s2_nhwc(CSplit16 in, Split16 out, int N, int H, int W, int C, cudaStream_t s);
 int launch_layernorm(CSplit16 x, const float* gamma, const float* beta, Split16 out, int rows, cudaStream_t s);
 // out = LN2(LN1(x)): the last decoder layer's norm3 followed by decoder.norm (transformer.py:110-111) in one pass

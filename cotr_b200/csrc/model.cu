@@ -310,7 +310,7 @@ struct Run {
 };
 
 enum KernelId { K_GEMM_TC = 0, K_GEMM_SIMT = 1, K_ATTN_TC = 2, K_ATTN_SIMT = 3, K_LAYERNORM = 4, K_MAXPOOL = 5, K_QENC = 6, K_STEM_CANVAS = 7,
-                K_GEMM_MLP = 8 };
+                K_GEMM_MLP = 8, K_ATTN_WEIGHTS_TC = 9, K_ATTN_WEIGHTS_SIMT = 10 };
 
 // Counts the launch and, when the profiler is on, brackets it with two events on the launching stream.
 struct LaunchScope {
@@ -457,6 +457,37 @@ int run_attention(const Run& r, const AttnParams& p) {
     return launch_attention_tc(p, r.s);
 }
 
+// Where the head-averaged attention maps of the selected layers go (cotr_encode_context_attention /
+// cotr_decode_attention): bit l of `mask` selects layer l, selected layers are stored one after the other in ascending
+// order, `base` is the first row of this call in the first selected layer's map.  mask = 0: no maps, no launches.
+struct AttnMaps {
+    unsigned mask = 0;
+    float* base = nullptr;
+    size_t layer_stride = 0;     // elements between the maps of consecutive selected layers
+    size_t pair_stride = 0;      // elements between the first rows of consecutive pairs
+    float* layer(int l) const {
+        if (!((mask >> l) & 1u)) return nullptr;
+        return base + (size_t)__builtin_popcount(mask & ((1u << l) - 1u)) * layer_stride;
+    }
+    AttnMaps at(size_t elems) const { AttnMaps a = *this; if (a.base) a.base += elems; return a; }
+};
+
+// The maps of one layer from the operands its attention launch `a` just read (attention_weights.cu); recorded like the
+// attention launch (M = query rows, N = 512 keys, K = 32 x 8 heads).
+int run_attention_weights(const Run& r, const AttnParams& a, const AttnMaps& maps, int layer) {
+    float* out = maps.layer(layer);
+    if (!out) return 0;
+    AttnWeightsParams p{};
+    p.q = a.q; p.ldq = a.ldq;
+    p.k = a.k; p.ldk = a.ldk;
+    p.kv_img = a.kv_img; p.img_pair_stride = a.img_pair_stride;
+    p.out = out; p.out_pair_stride = maps.pair_stride;
+    p.nq = a.nq; p.npairs = a.npairs; p.pair0 = a.pair0;
+    const bool tc = r.m->gemm_path == 0;
+    LaunchScope scope(r, tc ? K_ATTN_WEIGHTS_TC : K_ATTN_WEIGHTS_SIMT, a.nq * a.npairs, kTokens, kDModel);
+    return tc ? launch_attention_weights_tc(p, r.s) : launch_attention_weights_simt(p, r.s);
+}
+
 // ----------------------------------------------------------------------------------------------
 // workspace
 // ----------------------------------------------------------------------------------------------
@@ -582,7 +613,7 @@ int ensure_decode_ws(cotr_model* m, int rows) {
 // ----------------------------------------------------------------------------------------------
 // forward schedule
 // ----------------------------------------------------------------------------------------------
-int encode_impl(cotr_model* m, const float* img, int B, cotr_context* ctx, cudaStream_t s) {
+int encode_impl(cotr_model* m, const float* img, int B, cotr_context* ctx, cudaStream_t s, const AttnMaps& maps = AttnMaps()) {
     COTR_CHECK(B >= 1, "cotr_encode_context: B must be >= 1 (got %d)", B);
     COTR_CHECK(ctx && ctx->model == m, "cotr_encode_context: context does not belong to this model");
     COTR_CHECK(B <= ctx->max_pairs, "cotr_encode_context: B = %d exceeds the context capacity %d", B, ctx->max_pairs);
@@ -663,6 +694,7 @@ int encode_impl(cotr_model* m, const float* img, int B, cotr_context* ctx, cudaS
             a.out = w.ao; a.ldo = kDModel;
             a.nq = kTokens; a.npairs = B; a.pair0 = 0;
             if (run_attention(r, a)) return 1;
+            if (run_attention_weights(r, a, maps, l)) return 1;     // before the next layer overwrites qk / kvimg
             // xa = x + out_proj(attn)                                   (transformer.py:149-154, norm1 deferred)
             if (run_linear_dln(r, e.o, T, cs(w.ao), kDModel, w.xa, kDModel, false, nullptr, w.enc_st_a, cs(xin), kDModel,
                                ln_in ? w.enc_st_b : nullptr, ln_in ? m->enc[l - 1].ln2_g : nullptr, ln_in ? m->enc[l - 1].ln2_b : nullptr)) return 1;
@@ -718,6 +750,7 @@ int encode_impl(cotr_model* m, const float* img, int B, cotr_context* ctx, cudaS
         a.out = w.ao; a.ldo = kDModel;
         a.nq = kTokens; a.npairs = B; a.pair0 = 0;
         if (run_attention(r, a)) return 1;
+        if (run_attention_weights(r, a, maps, l)) return 1;         // before the next layer overwrites qk / kvimg
         // x1 = LN1(x + out_proj(attn))
         if (run_linear(r, e.o, T, cs(w.ao), kDModel, w.xa, kDModel, false, cs(xin), kDModel, e.ln1_g, e.ln1_b, w.ln_tmp)) return 1;
         // x2 = LN2(x1 + W2 relu(W1 x1 + b1) + b2)
@@ -754,8 +787,9 @@ int encode_impl(cotr_model* m, const float* img, int B, cotr_context* ctx, cudaS
     return 0;
 }
 
+// maps.base: this chunk's first row (pair pair0, its first query) in the caller's (n_sel, B, Q, 512) buffer
 int decode_chunk(cotr_model* m, const cotr_context* ctx, const float* queries, float* pred, int pair0, int npairs,
-                 int nq, cudaStream_t s) {
+                 int nq, cudaStream_t s, const AttnMaps& maps) {
     Workspace& w = m->ws;
     Run r{m, s};
     const int R = npairs * nq;
@@ -790,6 +824,7 @@ int decode_chunk(cotr_model* m, const cotr_context* ctx, const float* queries, f
             a.out = w.dao; a.ldo = kDModel;
             a.nq = nq; a.npairs = npairs; a.pair0 = pair0;
             if (run_attention(r, a)) return 1;
+            if (run_attention_weights(r, a, maps, l)) return 1;
             // transformer.py:196-197: t = t + out_proj(attn)   (norm2 deferred; t = norm3_{l-1}(t2), deferred, or 0)
             if (run_linear_dln(r, d.o, R, cs(w.dao), kDModel, w.t, kDModel, false, nullptr, w.dec_st_a, ln_in ? cs(w.t2) : none, kDModel,
                                ln_in ? w.dec_st_b : nullptr, ln_in ? m->dec[l - 1].ln3_g : nullptr, ln_in ? m->dec[l - 1].ln3_b : nullptr)) return 1;
@@ -822,6 +857,7 @@ int decode_chunk(cotr_model* m, const cotr_context* ctx, const float* queries, f
             a.out = w.dao; a.ldo = kDModel;
             a.nq = nq; a.npairs = npairs; a.pair0 = pair0;
             if (run_attention(r, a)) return 1;
+            if (run_attention_weights(r, a, maps, l)) return 1;
             // transformer.py:196-197: t = norm2(t + out_proj(attn))
             if (run_linear(r, d.o, R, cs(w.dao), kDModel, w.t, kDModel, false, l > 0 ? cs(w.t) : none, kDModel, d.ln2_g, d.ln2_b, w.dln_tmp)) return 1;
             // transformer.py:198-200: t = norm3(t + linear2(relu(linear1(t))))
@@ -852,7 +888,9 @@ int decode_chunk(cotr_model* m, const cotr_context* ctx, const float* queries, f
     return 0;
 }
 
-int decode_impl(cotr_model* m, const cotr_context* ctx, const float* queries, int B, int Q, float* pred, cudaStream_t s) {
+// maps (optional): base = attn_dev, layer_stride = B * Q * 512, pair_stride = Q * 512
+int decode_impl(cotr_model* m, const cotr_context* ctx, const float* queries, int B, int Q, float* pred, cudaStream_t s,
+                const AttnMaps& maps = AttnMaps()) {
     COTR_CHECK(ctx && ctx->model == m, "cotr_decode: context does not belong to this model");
     COTR_CHECK(B >= 1 && B == ctx->pairs, "cotr_decode: B = %d but the context holds %d pairs", B, ctx ? ctx->pairs : -1);
     COTR_CHECK(Q >= 0, "cotr_decode: negative Q");
@@ -867,14 +905,15 @@ int decode_impl(cotr_model* m, const cotr_context* ctx, const float* queries, in
         const int pairs_per = kDecodeChunkRows / Q;
         for (int b0 = 0; b0 < B; b0 += pairs_per) {
             const int nb = (B - b0 < pairs_per) ? B - b0 : pairs_per;
-            if (decode_chunk(m, ctx, queries + (size_t)b0 * Q * 2, pred + (size_t)b0 * Q * 2, b0, nb, Q, s)) return 1;
+            if (decode_chunk(m, ctx, queries + (size_t)b0 * Q * 2, pred + (size_t)b0 * Q * 2, b0, nb, Q, s,
+                             maps.at((size_t)b0 * Q * kTokens))) return 1;
         }
     } else {
         for (int b = 0; b < B; ++b)
             for (int q0 = 0; q0 < Q; q0 += kDecodeChunkRows) {
                 const int nq = (Q - q0 < kDecodeChunkRows) ? Q - q0 : kDecodeChunkRows;
                 const size_t off = ((size_t)b * Q + q0) * 2;
-                if (decode_chunk(m, ctx, queries + off, pred + off, b, 1, nq, s)) return 1;
+                if (decode_chunk(m, ctx, queries + off, pred + off, b, 1, nq, s, maps.at(((size_t)b * Q + q0) * kTokens))) return 1;
             }
     }
     m->last_rows = (total <= kDecodeChunkRows) ? (int)total : 0;
@@ -1154,6 +1193,44 @@ int cotr_decode(cotr_model* m, const cotr_context* ctx, const float* queries_dev
     CallOrder order(m, (cudaStream_t)cuda_stream);
     m->launches = 0;
     return decode_impl(m, ctx, queries_dev, B, Q, pred_dev, (cudaStream_t)cuda_stream);
+}
+
+namespace {
+int check_layer_mask(const char* fn, int layer_mask, const float* attn_dev, int n_layers) {
+    COTR_CHECK((layer_mask & ~((1 << n_layers) - 1)) == 0, "%s: layer_mask 0x%x selects layers outside 0..%d", fn, (unsigned)layer_mask, n_layers - 1);
+    COTR_CHECK(layer_mask == 0 || attn_dev != nullptr, "%s: null attn_dev for layer_mask 0x%x", fn, (unsigned)layer_mask);
+    return 0;
+}
+}  // namespace
+
+int cotr_encode_context_attention(cotr_model* m, const float* img_dev, int B, cotr_context* ctx, int layer_mask, float* attn_dev,
+                                  void* cuda_stream) {
+    COTR_CHECK(m && img_dev, "cotr_encode_context_attention: null argument");
+    if (check_layer_mask("cotr_encode_context_attention", layer_mask, attn_dev, kEncLayers)) return 1;
+    COTR_CHECK_CUDA(cudaSetDevice(m->device));
+    CallOrder order(m, (cudaStream_t)cuda_stream);
+    m->launches = 0;
+    AttnMaps maps;
+    maps.mask = (unsigned)layer_mask;
+    maps.base = attn_dev;
+    maps.layer_stride = (size_t)B * kTokens * kTokens;
+    maps.pair_stride = (size_t)kTokens * kTokens;
+    return encode_impl(m, img_dev, B, ctx, (cudaStream_t)cuda_stream, maps);
+}
+
+int cotr_decode_attention(cotr_model* m, const cotr_context* ctx, const float* queries_dev, int B, int Q, int layer_mask,
+                          float* attn_dev, float* pred_dev, void* cuda_stream) {
+    COTR_CHECK(m && (Q == 0 || (queries_dev && pred_dev)), "cotr_decode_attention: null argument");
+    if (check_layer_mask("cotr_decode_attention", layer_mask, attn_dev, kDecLayers)) return 1;
+    COTR_CHECK_CUDA(cudaSetDevice(m->device));
+    CallOrder order(m, (cudaStream_t)cuda_stream);
+    m->launches = 0;
+    AttnMaps maps;
+    maps.mask = (unsigned)layer_mask;
+    maps.base = attn_dev;
+    maps.layer_stride = (size_t)B * Q * kTokens;
+    maps.pair_stride = (size_t)Q * kTokens;
+    return decode_impl(m, ctx, queries_dev, B, Q, pred_dev, (cudaStream_t)cuda_stream, maps);
 }
 
 namespace {
@@ -1591,6 +1668,55 @@ int cotr_test_attention(int path, const float* q_dev, const float* k_dev, const 
     cudaError_t e = cudaDeviceSynchronize();
     if (rc) return rc;
     COTR_CHECK(e == cudaSuccess, "cotr_test_attention: kernel failed: %s", cudaGetErrorString(e));
+    return 0;
+}
+
+// q (npairs*nq,256), k (npairs*512,256) fp32 row-major -> out (npairs,nq,512).  Path 0 reads k as the attention operand
+// images, written by the same epilogue store (split16.cuh store16) as in the model, through an identity "GEMM".
+int cotr_test_attention_weights(int path, const float* q_dev, const float* k_dev, float* out_dev, int nq, int npairs) {
+    COTR_CHECK(q_dev && k_dev && out_dev, "cotr_test_attention_weights: null argument");
+    COTR_CHECK(nq >= 1 && npairs >= 1, "cotr_test_attention_weights: nq and npairs must be >= 1");
+    TmpSplit q16, k16;
+    const size_t qn = (size_t)npairs * nq * kDModel, kn = (size_t)npairs * kTokens * kDModel;
+    if (q16.from_f32(q_dev, qn) || k16.from_f32(k_dev, kn)) return 1;
+    AttnWeightsParams a{};
+    a.q = cs(q16.t); a.ldq = kDModel;
+    a.out = out_dev; a.out_pair_stride = (size_t)nq * kTokens;
+    a.nq = nq; a.npairs = npairs; a.pair0 = 0;
+    unsigned char* img = nullptr;
+    int rc = 0;
+    if (path == 0) {
+        COTR_CHECK_CUDA(cudaMalloc((void**)&img, (size_t)npairs * kHeads * kAttnHeadImgBytes));
+        std::vector<float> eye((size_t)kDModel * kDModel, 0.f);
+        for (int i = 0; i < kDModel; ++i) eye[(size_t)i * kDModel + i] = 1.f;
+        std::vector<uint8_t> eye_tc(tc_weight_bytes(kDModel, kDModel));
+        const float eye_scale = tc_pack_weight(eye.data(), kDModel, kDModel, eye_tc.data());
+        void* wtc = nullptr;
+        rc = cudaMalloc(&wtc, eye_tc.size()) != cudaSuccess ||
+             cudaMemcpy(wtc, eye_tc.data(), eye_tc.size(), cudaMemcpyHostToDevice) != cudaSuccess ||
+             cudaMemset(img, 0, (size_t)npairs * kHeads * kAttnHeadImgBytes) != cudaSuccess;
+        if (rc) set_error("cotr_test_attention_weights: device allocation failed");
+        if (!rc) {      // the key blocks of the tensor-core GEMM epilogue go into the operand images
+            GemmParams p;
+            memset(&p, 0, sizeof(p));
+            p.M = npairs * kTokens; p.N = kDModel; p.K = kDModel;
+            p.a = cs(k16.t); p.a_mode = A_ROWMAJOR; p.lda = kDModel;
+            p.Wtc = wtc; p.acc_scale = eye_scale; p.add_period = 1;
+            p.remap = 1; p.blk_map[0] = -1000; p.n_vt = 1; p.kv_img = img; p.ldc = kDModel;
+            rc = launch_gemm_tc(p, 0);
+        }
+        cudaDeviceSynchronize();
+        if (wtc) cudaFree(wtc);
+        a.kv_img = img; a.img_pair_stride = (size_t)kHeads * kAttnHeadImgBytes;
+        if (!rc) rc = launch_attention_weights_tc(a, 0);
+    } else {
+        a.k = cs(k16.t); a.ldk = kDModel;
+        rc = launch_attention_weights_simt(a, 0);
+    }
+    const cudaError_t e = cudaDeviceSynchronize();
+    if (img) cudaFree(img);
+    if (rc) return rc;
+    COTR_CHECK(e == cudaSuccess, "cotr_test_attention_weights: kernel failed: %s", cudaGetErrorString(e));
     return 0;
 }
 

@@ -11,6 +11,20 @@ Reference contract (COTR/models/cotr_model.py:17-51):
 The arithmetic is NOT done by torch: forward hands device pointers to libcotr_b200.so (include/cotr_b200.h).
 There is no CPU path; calling forward without a CUDA device or without the built library raises.
 Unlike the reference constructor (backbone.py:106 `pretrained=True`) nothing is downloaded.
+
+Attention maps: the reference calls every transformer.encoder.layers[l].self_attn and
+transformer.decoder.layers[l].multihead_attn with need_weights=True (transformer.py:149-153, :192-195), so a forward
+hook on one of them sees the head-averaged attention weights as output[1].  Here those modules are parameter
+containers that are never called, so `forward` looks for forward hooks (plain and with_kwargs) on them itself: when
+there are any, it runs the native entry points that also compute the maps of exactly the hooked layers
+(cotr_encode_context_attention / cotr_decode_attention) and then calls each hook as torch would, in the reference's
+firing order (encoder layers 0..5, then decoder layers 0..5), with args = () (the reference passes only keywords),
+kwargs = {} for with_kwargs hooks, and output = (None, weights): weights is (B, 512, 512) for an encoder layer and
+(B, Q, 512) for a decoder layer, fp32 on the module's device; output[0], the attention output, is None because it is
+never materialised.  A hook's return value is ignored.  `encode_context` fires the encoder hooks and `decode` the
+decoder hooks, so a caller that encodes once and decodes twice (cotr_corr_base's cycle pass) sees the encoder hooks
+fire once where the reference fires them twice.  Without hooks nothing of this runs.  Forward pre-hooks and the
+sharded model are not covered.
 """
 import math
 
@@ -170,12 +184,16 @@ class COTR(nn.Module):
         self.backbone = backbone
         self._native = None
         self._ctx_cache = {}
+        self._hook_ctx = None                     # context of hooked forwards (grown to the largest batch seen)
 
     # ---- native handle management ---------------------------------------------------------------------
     def _invalidate(self):
         for ctx in self._ctx_cache.values():
             ctx.close()
         self._ctx_cache = {}
+        if self._hook_ctx is not None:
+            self._hook_ctx.close()
+        self._hook_ctx = None
         if self._native is not None:
             self._native.close()
         self._native = None
@@ -223,11 +241,63 @@ class COTR(nn.Module):
         assert q.ndim == 3 and q.shape[-1] == 2 and q.shape[0] == batch, f"queries must be (B,Q,2), got {tuple(q.shape)}"
         return q
 
+    # ---- forward hooks on the attention containers (see the module docstring) ---------------------------------
+    def _attention_modules(self):
+        t = self.transformer
+        return ([getattr(t.encoder.layers, str(l)).self_attn for l in range(6)],
+                [getattr(t.decoder.layers, str(l)).multihead_attn for l in range(6)])
+
+    @staticmethod
+    def _hooked(mods):
+        """bit l set: module l has at least one forward hook"""
+        return sum(1 << l for l, m in enumerate(mods) if m._forward_hooks)
+
+    @staticmethod
+    def _fire(mods, mask, maps):
+        n = 0
+        for l, m in enumerate(mods):
+            if not (mask >> l) & 1:
+                continue
+            output = (None, maps[n])
+            n += 1
+            for hook_id, hook in list(m._forward_hooks.items()):
+                if m._forward_hooks_with_kwargs.get(hook_id, False):
+                    hook(m, (), {}, output)
+                else:
+                    hook(m, (), output)
+
+    def _encode(self, x, native_ctx):
+        nat = self.native()
+        enc, _ = self._attention_modules()
+        mask = self._hooked(enc)
+        if not mask:
+            nat.encode_context(x, native_ctx)
+            return
+        self._fire(enc, mask, nat.encode_context_attention(x, native_ctx, mask))
+
+    def _decode(self, native_ctx, q):
+        nat = self.native()
+        _, dec = self._attention_modules()
+        mask = self._hooked(dec)
+        if not mask:
+            return nat.decode(native_ctx, q)
+        pred, maps = nat.decode_attention(native_ctx, q, mask)
+        self._fire(dec, mask, maps)
+        return pred
+
     @torch.no_grad()
     def forward(self, samples, queries):
         x = self._canvas(samples)
         q = self._queries(queries, x.shape[0])
-        return {'pred_corrs': self.native().forward(x, q)}
+        enc, dec = self._attention_modules()
+        if not (self._hooked(enc) or self._hooked(dec)):
+            return {'pred_corrs': self.native().forward(x, q)}
+        if self._hook_ctx is None or self._hook_ctx.max_pairs < x.shape[0]:
+            if self._hook_ctx is not None:
+                self._hook_ctx.close()
+            self._hook_ctx = capi.NativeContext(self.native(), x.shape[0])
+        self._encode(x, self._hook_ctx)
+        return {'pred_corrs': self._decode(self._hook_ctx, q)}
 
     # ---- extensions used by cotr_b200.inference ---------------------------------------------------------
     supports_device_preprocess = True
@@ -271,13 +341,13 @@ class COTR(nn.Module):
         else:
             native_ctx = capi.NativeContext(nat, x.shape[0])
         ctx = Context(native_ctx, x.shape[0])
-        nat.encode_context(x, ctx.native)
+        self._encode(x, ctx.native)
         return ctx
 
     @torch.no_grad()
     def decode(self, ctx, queries):
         q = self._queries(queries, ctx.batch)
-        return {'pred_corrs': self.native().decode(ctx.native, q)}
+        return {'pred_corrs': self._decode(ctx.native, q)}
 
 
 def build(args):

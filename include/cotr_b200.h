@@ -74,6 +74,21 @@ int cotr_encode_context(cotr_model* m, const float* img_dev, int B, cotr_context
 int cotr_decode(cotr_model* m, const cotr_context* ctx, const float* queries_dev, int B, int Q,
                 float* pred_dev, void* cuda_stream);
 
+/* The same two calls, also returning the head-averaged attention maps of the layers selected by `layer_mask` (bit l =
+ * layer l, 0..5): the second output of the reference's nn.MultiheadAttention (need_weights=True), i.e. what a forward
+ * hook on transformer.encoder.layers[l].self_attn / transformer.decoder.layers[l].multihead_attn sees as output[1].
+ * attn_dev [b][i][j] = (1/8) sum over heads h = 0..7 of softmax_j(q_h[i] . k_h[j]), key j = token row * 32 + col of the
+ * 16 x 32 context grid (col < 16: left image), fp32, selected layers stored in ascending order:
+ *   cotr_encode_context_attention: attn_dev (popcount(layer_mask), B, 512, 512)
+ *   cotr_decode_attention:         attn_dev (popcount(layer_mask), B, Q, 512)
+ * layer_mask = 0 is exactly the plain call (attn_dev may be NULL); bits at 6 or above, or a NULL attn_dev with a
+ * non-zero mask, fail.  Contexts and predictions are bitwise those of the plain calls: each selected layer adds one
+ * launch that only reads.  Both calls run eagerly (no CUDA-graph capture). */
+int cotr_encode_context_attention(cotr_model* m, const float* img_dev, int B, cotr_context* ctx, int layer_mask,
+                                  float* attn_dev, void* cuda_stream);
+int cotr_decode_attention(cotr_model* m, const cotr_context* ctx, const float* queries_dev, int B, int Q, int layer_mask,
+                          float* attn_dev, float* pred_dev, void* cuda_stream);
+
 /* cotr_encode_context + cotr_decode on an internal context. */
 int cotr_forward(cotr_model* m, const float* img_dev, const float* queries_dev, int B, int Q,
                  float* pred_dev, void* cuda_stream);
@@ -172,7 +187,9 @@ int cotr_last_launch_count(const cotr_model* m);
  * by two CUDA events recorded on the launching stream.  cotr_profile_end synchronises the device, fills `out` with
  * one record per launch in launch order and returns -(count + 1) on success (so 0 records -> -1), > 0 on failure.
  * kernel ids: 0 gemm_tc (wgmma), 1 gemm_simt, 2 attention_tc, 3 attention_simt, 4 layernorm, 5 maxpool,
- * 6 query_encode, 7 stem_canvas.  For GEMMs M,N,K are the problem size; for attention M = query rows, N = 512, K = 256. */
+ * 6 query_encode, 7 stem_canvas, 8 gemm_mlp (fused feed-forward block), 9 attention_weights_tc, 10 attention_weights_simt
+ * (the maps of cotr_*_attention).  For GEMMs M,N,K are the problem size; for attention and attention weights
+ * M = query rows, N = 512, K = 256. */
 typedef struct cotr_launch_record {
     int32_t kernel;
     int32_t M, N, K;
@@ -216,6 +233,9 @@ int cotr_test_gemm(const cotr_test_gemm_desc* d, const float* A_dev, const float
 /* out[(p*nq+i), h*32+d] = softmax(q k^T) v per head; q (npairs*nq,256), k/v (npairs*512,256), all DEVICE, ld 256. */
 int cotr_test_attention(int path, const float* q_dev, const float* k_dev, const float* v_dev, float* out_dev,
                         int nq, int npairs);
+/* out[(p*nq+i), j] = head-averaged softmax(q k^T) (the maps of cotr_decode_attention); q (npairs*nq,256), k (npairs*512,256),
+ * out (npairs,nq,512), all DEVICE.  Path 0 reads k through the attention operand images, path 1 row-major. */
+int cotr_test_attention_weights(int path, const float* q_dev, const float* k_dev, float* out_dev, int nq, int npairs);
 /* bring-up / A-B switches (0 = production): bit 8 (256) disables programmatic dependent launch, bit 9 (512) disables
  * split-K, bits 10-11 move the CTA-count threshold of the 64-wide GEMM tile, bits 14-15 lower the
  * minimum K of split-K (16 >> n chunks of 64).  Schedule: by default a transformer section with >= 2048 rows runs the
