@@ -55,18 +55,49 @@ constexpr int kBarConsumers = 6;        // named barrier of the 8 consumer warps
 // CTAs of about one wave on the 132 SMs of an H100 SXM (one CTA per SM: the pipeline takes most of shared memory)
 constexpr long long kWaveCtas = 144;
 
-enum LoaderMode : int { LD_GATHER = 0, LD_CONV = 1, LD_STEM4 = 2 };
+enum LoaderMode : int { LD_GATHER = 0, LD_CONV = 1, LD_STEM4 = 2, LD_HALO = 3 };
 
 __host__ __device__ inline int tc_npad(int N) { return N >= 64 ? ((N + 63) / 64) * 64 : ((N + 15) / 16) * 16; }
 
-template <int BN>
+// Halo loader (LD_HALO) of the 3x3 stride-1 convolutions.  The implicit im2col stages a 128 x 64 A tile per (tap,
+// 64-channel) chunk, i.e. every input pixel nine times.  Instead, the output rows of an image are numbered over the
+// zero-padded (H+2) x (W+2) grid, m = oh (W+2) + ow with ow in [0, W+2) (rows with ow >= W, and those past the last
+// output row, are computed and dropped by the epilogue; tiles never cross images), so that tap (kh, kw) of output row m
+// is padded input position m + kh (W+2) + kw.  A tile of 128 rows starting at q0 then needs the padded positions
+// [q0, q0 + 128 + 2 (W+2) + 2) of each 64-channel chunk: the producer stages them ONCE (zero-filled outside the image,
+// SWIZZLE_128B keyed by the absolute halo row) and they stay resident; tap (kh, kw) is the view of that tile at row
+// offset kh (W+2) + kw: a plain make_desc_sw128 of the view's address, base-offset field 0 (the unit applies the
+// 128-byte swizzle to the absolute shared-memory address bits, so a view that starts at any row keeps the tile's
+// phase; checked on H100 for row offsets 0..23, whereas base offset (addr >> 7) & 7 is wrong).  Only the weights
+// stream through the pipeline stages.  The K order is the implicit im2col's (tap-major, channel-minor); split-K
+// hands each CTA of the cluster whole channel chunks.
+constexpr uint32_t kHaloMaxBytes = 100u * 1024u;        // resident halo tiles of one CTA (both planes, all its chunks)
+constexpr int kHaloMaxChunks = 4;
+constexpr long long kHaloMinCtas = 86;                  // two thirds of the 132 SMs (see launch_one)
+__host__ __device__ inline int halo_pitch(const GemmParams& p) { return p.W + 2; }
+__host__ __device__ inline int halo_tiles_per_img(const GemmParams& p) { return (p.OH * halo_pitch(p) + 127) / 128; }
+__host__ __device__ inline int halo_rows(const GemmParams& p) { return 128 + 2 * halo_pitch(p) + 2; }
+__host__ __device__ inline uint32_t halo_plane_bytes(const GemmParams& p) { return (uint32_t)((halo_rows(p) + 7) / 8 * 8) * 128u; }
+// dense NHWC output row of padded-grid row m, or -1 for the rows the halo grid adds
+__device__ __forceinline__ int halo_out_row(const GemmParams& p, int m) {
+    const int tpi = halo_tiles_per_img(p), pitch = halo_pitch(p);
+    const int tile = m >> 7, n = tile / tpi;
+    const int local = (tile - n * tpi) * 128 + (m & 127);
+    const int oh = local / pitch, ow = local - oh * pitch;
+    return (oh < p.OH && ow < p.OW) ? (n * p.OH + oh) * p.OW + ow : -1;
+}
+
+template <int BN, int MODE = LD_GATHER>
 struct Cfg {
     static constexpr int BM = BN >= 256 ? 64 : 128;
     static constexpr int WN = BN >= 256 ? 128 : BN;                     // columns of one consumer warpgroup's wgmma
     static constexpr uint32_t kAPlane = BM * 128u;                      // one fp16 plane (hi or lo) of the BM x 64 A tile
     static constexpr uint32_t kBPlane = BN * 128u;                      // BN rows x 128 bytes
-    static constexpr uint32_t kStage = 2 * kAPlane + 2 * kBPlane;
-    static constexpr int kStagesRaw = (int)((227u * 1024u - 3072u) / kStage);
+    // LD_HALO: the A halo tiles sit in their own region in front of the stages, which then carry the weights only
+    static constexpr uint32_t kHaloBytes = MODE == LD_HALO ? kHaloMaxBytes : 0u;
+    static constexpr uint32_t kAStage = MODE == LD_HALO ? 0u : 2 * kAPlane;
+    static constexpr uint32_t kStage = kAStage + 2 * kBPlane;
+    static constexpr int kStagesRaw = (int)((227u * 1024u - 3072u - kHaloBytes) / kStage);
     static constexpr int kStages = kStagesRaw > 4 ? 4 : kStagesRaw;
     // register accumulators of one warpgroup (WN / 2 floats per thread each): kMain slots take the hi*hi products
     // round-robin over the k16 steps, kCorr slots the lo*hi / hi*lo products
@@ -88,9 +119,9 @@ struct Cfg {
     static constexpr int kRing = kChunksW < 2 ? kChunksW : 2;
     // behind the stages: 256 bytes of barriers, then the per-column vectors of the deferred LayerNorm (column sums of
     // W' or gamma | beta of this tile's BN columns, staged by two producer warps while the main loop runs), then split-K partials
-    static constexpr uint32_t kVecOffset = kStages * kStage + 256;
+    static constexpr uint32_t kVecOffset = kStages * kStage + 256;       // (offsets behind the halo region)
     static constexpr uint32_t kVecBytes = 2u * BN * 4u + 2u * BM * 8u;   // + (mean, rstd) of the BM A rows and of the BM residual rows
-    static constexpr uint32_t kSmemBytes = kStages * kStage + 2048 + kVecBytes;     // + alignment slack + barriers + vectors
+    static constexpr uint32_t kSmemBytes = kHaloBytes + kStages * kStage + 2048 + kVecBytes;     // + alignment slack + barriers + vectors
     // split-K (reduce-scatter over the rows): every CTA of the cluster finishes 128 / ksplit rows of the tile and
     // receives the other CTAs' fp32 partial rows behind the barriers (a dedicated region, so peers may push while this
     // CTA's pipeline is still running); rows of BN * 4 bytes, 16-byte pieces XOR-swizzled by row % 8 (thread-per-row
@@ -101,8 +132,8 @@ struct Cfg {
     static constexpr uint32_t kPartMaxBytes = kMaxSplit > 1 ? 96u * kPartPitch : 0u;   // ksplit 4: 3 x 32 rows; 2: 1 x 64 rows
     static_assert(kSmemBytes + kPartMaxBytes <= 227u * 1024u, "split-K partial tiles do not fit");
     static_assert(kStages >= 2, "pipeline needs at least two stages");
-    static_assert(kAccTileBytes + (BM / 32) * kWarpStaging <= kStages * kStage, "epilogue tiles do not fit the idle stages");
-    static_assert(kStage % 1024 == 0 && kAPlane % 1024 == 0, "stages must stay 1024-byte aligned for SWIZZLE_128B");
+    static_assert(kAccTileBytes + (BM / 32) * kWarpStaging <= kHaloBytes + kStages * kStage, "epilogue tiles do not fit the idle stages");
+    static_assert(kStage % 1024 == 0 && kAPlane % 1024 == 0 && kHaloBytes % 1024 == 0, "stages must stay 1024-byte aligned for SWIZZLE_128B");
     static_assert(kMaxSplit == 1 || BM == 128, "split-K hands over 32-row groups of a 128-row tile");
 };
 
@@ -117,21 +148,23 @@ struct EpiOperands {
 // The default schedule uses DLN = false kernels, which contain none of it.
 template <int BN, bool LN, int MODE, bool DLN>
 __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const GemmParams p, const int npad) {
-    using C = Cfg<BN>;
+    using C = Cfg<BN, MODE>;
     constexpr int BM = C::BM;
     extern __shared__ uint8_t smem_raw[];
     const uint32_t raw_addr = smem_u32(smem_raw);
-    uint8_t* stage_base = smem_raw + (((raw_addr + 1023u) & ~1023u) - raw_addr);      // SWIZZLE_128B needs 1024-byte alignment
+    uint8_t* tile_mem = smem_raw + (((raw_addr + 1023u) & ~1023u) - raw_addr);        // SWIZZLE_128B needs 1024-byte alignment
+    uint8_t* stage_base = tile_mem + C::kHaloBytes;                                     // LD_HALO: behind the resident halo tiles
     uint64_t* bars = reinterpret_cast<uint64_t*>(stage_base + C::kStages * C::kStage);
     uint64_t* full_a = bars;
     uint64_t* empty = bars + C::kStages;
     uint64_t* part_full = bars + 2 * C::kStages;           // split-K leader: all peers' partial tiles have landed
     uint64_t* vec_full = bars + 2 * C::kStages + 1;        // deferred LayerNorm: the per-column vectors are staged
+    uint64_t* halo_full = bars + 2 * C::kStages + 2;       // LD_HALO: halo tile c of this CTA has landed
     float* vec_a = reinterpret_cast<float*>(stage_base + C::kVecOffset);      // a_ln: column sums of W'; res_ln: gamma
     float* vec_b = vec_a + BN;                                                  //                         res_ln: beta
     float2* st_a = reinterpret_cast<float2*>(vec_b + BN);                       // (mean, rstd) of the A rows of this tile
     float2* st_r = st_a + BM;                                                   // (mean, rstd) of the residual rows
-    float* acc_tile = reinterpret_cast<float*>(stage_base);                     // epilogue: summed accumulators [BM][kAccPitch]
+    float* acc_tile = reinterpret_cast<float*>(tile_mem);                       // epilogue: summed accumulators [BM][kAccPitch]
     // deferred LayerNorm (GemmParams::a_ln_cs / res_ln_part / ln_part_out): only the row-major loader instantiations carry it
     static_assert(!DLN || (MODE == LD_GATHER && !LN), "deferred LayerNorm: row-major operand tiles only");
     constexpr bool kCanLnA = DLN;
@@ -150,12 +183,25 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const GemmParams p
     const int kz = blockIdx.z;
     const int KC = ((p.K + BK - 1) / BK) / ksplit;
     const int it0 = kz * KC;
+    // LD_HALO: this CTA's channel chunks [kz ccp, (kz+1) ccp) of cc; iteration it = tap * ccp + chunk
+    const int cc = p.C / BK, ccp = cc / ksplit;
+    const uint32_t halo_plane = MODE == LD_HALO ? halo_plane_bytes(p) : 0u;
+    // weight image chunk of iteration it (k = tap * C + channel)
+    auto w_chunk = [&](int it) {
+        if constexpr (MODE == LD_HALO) {
+            const int tap = it / ccp;
+            return tap * cc + kz * ccp + (it - tap * ccp);
+        }
+        return it0 + it;
+    };
 
     if (threadIdx.x == 0) {
         for (int s = 0; s < C::kStages; ++s) {
-            mbar_init(&full_a[s], 129);
+            mbar_init(&full_a[s], MODE == LD_HALO ? 1 : 129);      // (128 loader arrivals) + 1 expect_tx
             mbar_init(&empty[s], 8);          // one arrival per consumer warp
         }
+        if (MODE == LD_HALO)
+            for (int c = 0; c < ccp; ++c) mbar_init(&halo_full[c], 128);
         mbar_init(part_full, 1);
         if (DLN) mbar_init(vec_full, 64);
         mbar_fence_init();
@@ -176,8 +222,8 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const GemmParams p
         auto load_weights = [&](int it) {
             const int s = it % C::kStages;
             mbar_arrive_expect_tx(&full_a[s], 2u * C::kBPlane);
-            uint8_t* b_dst = stage_base + (size_t)s * C::kStage + 2 * C::kAPlane;
-            const uint8_t* src = wimg + (((size_t)(it0 + it) * 2) * npad + n0) * 128;
+            uint8_t* b_dst = stage_base + (size_t)s * C::kStage + C::kAStage;
+            const uint8_t* src = wimg + (((size_t)w_chunk(it) * 2) * npad + n0) * 128;
             tma_bulk_g2s(b_dst, src, C::kBPlane, &full_a[s]);
             tma_bulk_g2s(b_dst + C::kBPlane, src + (size_t)npad * 128, C::kBPlane, &full_a[s]);
         };
@@ -195,8 +241,10 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const GemmParams p
             }
         }
         ARow rows[kRowIters];
+        if constexpr (MODE != LD_HALO) {
 #pragma unroll
-        for (int i = 0; i < kRowIters; ++i) rows[i] = decode_a_row(p, m0 + rb + 16 * i);
+            for (int i = 0; i < kRowIters; ++i) rows[i] = decode_a_row(p, m0 + rb + 16 * i);
+        }
         const uint32_t a_off = (uint32_t)rb * 128u + (uint32_t)((kg ^ (rb & 7)) << 4);   // swizzled chunk position
         const uint32_t dst0 = smem_u32(stage_base) + a_off;
         // Weights are constants: the first stages' copies overlap the previous kernel.  Then let the next kernel of the
@@ -208,12 +256,36 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const GemmParams p
         }
         pdl_wait();
 
+        if constexpr (MODE == LD_HALO) {
+            // the halo tiles of this CTA's channel chunks, once: halo row j = padded input position q0 + j of image n
+            const int pitch = halo_pitch(p), tpi = halo_tiles_per_img(p), hrows = halo_rows(p);
+            const int n = blockIdx.x / tpi, q0 = (blockIdx.x - n * tpi) * 128;
+            const size_t img = (size_t)n * p.H * p.W * p.C;
+            for (int c = 0; c < ccp; ++c) {
+                const int ch = (kz * ccp + c) * BK + kg * 8;
+                const uint32_t dst = smem_u32(tile_mem) + (uint32_t)c * 2u * halo_plane;
+#pragma unroll 4
+                for (int j = rb; j < hrows; j += 16) {
+                    const int q = q0 + j;
+                    const int ih = q / pitch - 1, iw = q - (ih + 1) * pitch - 1;
+                    const bool ok = ih >= 0 && ih < p.H && iw >= 0 && iw < p.W;
+                    const size_t off = ok ? img + ((size_t)ih * p.W + iw) * p.C + ch : 0;
+                    const uint32_t d = dst + (uint32_t)j * 128u + (uint32_t)((kg ^ (j & 7)) << 4);
+                    cp_async16(d, p.a.hi + off, ok ? 16u : 0u);
+                    cp_async16(d + halo_plane, p.a.lo + off, ok ? 16u : 0u);
+                }
+                cp_async_mbar_arrive_noinc(&halo_full[c]);
+            }
+        }
+
 #pragma unroll 1
         for (int it = 0; it < KC; ++it) {
+            // (every producer thread walks the loop, so that the warps reach the final __syncthreads converged)
             const int s = it % C::kStages;
             const uint32_t ph = (uint32_t)(it / C::kStages) & 1u;
             mbar_wait(&empty[s], ph ^ 1u);
             if (t == 0 && it >= C::kStages) load_weights(it);
+            if constexpr (MODE == LD_HALO) continue;             // the stages carry weights only
             const int k0 = (it0 + it) * BK;
             {
                 const uint32_t dst = dst0 + (uint32_t)s * C::kStage;
@@ -323,17 +395,24 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const GemmParams p
         for (int it = 0; it < KC; ++it) {
             const int s = it % C::kStages;
             const uint32_t ph = (uint32_t)(it / C::kStages) & 1u;
+            uint32_t a_addr = smem_u32(stage_base + (size_t)s * C::kStage);
+            uint32_t a_plane = C::kAPlane;
+            if constexpr (MODE == LD_HALO) {                   // tap (kh, kw) = the halo tile seen kh (W+2) + kw rows further down
+                const int tap = it / ccp, c = it - tap * ccp, kh = tap / 3;
+                mbar_wait(&halo_full[c], 0);
+                a_plane = halo_plane;
+                a_addr = smem_u32(tile_mem) + (uint32_t)c * 2u * halo_plane + (uint32_t)(kh * halo_pitch(p) + tap - 3 * kh) * 128u;
+            }
             mbar_wait(&full_a[s], ph);
             fence_proxy_async_smem();                          // cp.async (generic proxy) data -> wgmma (async proxy)
-            const uint32_t a_addr = smem_u32(stage_base + (size_t)s * C::kStage);
-            const uint32_t b_addr = a_addr + 2 * C::kAPlane;
+            const uint32_t b_addr = smem_u32(stage_base + (size_t)s * C::kStage) + C::kAStage;
             fence_all();
             wgmma_fence();
 #pragma unroll
             for (int ks = 0; ks < BK / 16; ++ks) {
                 // a k16 step = 32 bytes inside the 128-byte swizzle atom
                 const uint64_t dah = make_desc_sw128(a_addr + a_sub + 32 * ks);
-                const uint64_t dal = make_desc_sw128(a_addr + C::kAPlane + a_sub + 32 * ks);
+                const uint64_t dal = make_desc_sw128(a_addr + a_plane + a_sub + 32 * ks);
                 const uint64_t dbh = make_desc_sw128(b_addr + b_sub + 32 * ks);
                 const uint64_t dbl = make_desc_sw128(b_addr + C::kBPlane + b_sub + 32 * ks);
                 mma(acc_c[0], dal, dbh);
@@ -496,7 +575,7 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const GemmParams p
         // fp32 prediction head keep the direct path.
         size_t tile_base = 0;
         const bool direct = p.out_f32 != nullptr || out_location(p, m0, n0, tile_base);
-        uint8_t* const stg_base = stage_base + C::kAccTileBytes;          // behind the accumulator tile
+        uint8_t* const stg_base = tile_mem + C::kAccTileBytes;            // behind the accumulator tile
         uint8_t* stg = stg_base + (uint32_t)ew * C::kWarpStaging + (uint32_t)lane * C::kOutPitch;
         auto emit16 = [&](int c, const float (&v)[16]) {          // c = column inside the tile
             if (direct) {
@@ -521,17 +600,23 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const GemmParams p
             const uint8_t* wbase = stg_base + (uint32_t)ew * C::kWarpStaging;
             const int r_in = kLanesPerRow >= 32 ? 0 : lane / kLanesPerRow;
             const int piece0 = kLanesPerRow >= 32 ? lane : lane % kLanesPerRow;
-            __half* gout = (plane == 0 ? p.out.hi : p.out.lo) + tile_base;     // element (m0, n0 mapped)
+            __half* gout = plane == 0 ? p.out.hi : p.out.lo;
 #pragma unroll 4
             for (int r0 = 0; r0 < 32; r0 += kRowsPerPass) {
                 const int rr = r0 + r_in;
                 const int grow_ = m0 + ew * 32 + rr;
+                bool ok = grow_ < p.M;
+                size_t roff = tile_base + (size_t)(ew * 32 + rr) * p.ldc;          // element (row, n0 mapped)
+                if constexpr (MODE == LD_HALO) {               // padded-grid row -> dense NHWC row; the grid's extra rows are dropped
+                    const int orow = halo_out_row(p, grow_);
+                    ok = orow >= 0;
+                    roff = (size_t)orow * p.ldc + n0;
+                }
 #pragma unroll
                 for (int q = 0; q < kPiecesPerLane; ++q) {
                     const int piece = piece0 + q * 32;
                     const uint4 val = *reinterpret_cast<const uint4*>(wbase + (uint32_t)(plane * 32 + rr) * C::kOutPitch + piece * 16);
-                    if (grow_ < p.M)
-                        *reinterpret_cast<uint4*>(gout + (size_t)(ew * 32 + rr) * p.ldc + piece * 8) = val;
+                    if (ok) *reinterpret_cast<uint4*>(gout + roff + piece * 8) = val;
                 }
             }
         };
@@ -683,24 +768,40 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const GemmParams p
 
 template <int BN, bool LN, int MODE, bool DLN = false>
 int launch_one(const GemmParams& p, cudaStream_t s) {
-    using C = Cfg<BN>;
+    using C = Cfg<BN, MODE>;
     static unsigned long long configured = 0;      // bit per device
     if (first_use_on_device(&configured)) {
         COTR_CHECK_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<BN, LN, MODE, DLN>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                              (int)(C::kSmemBytes + C::kPartMaxBytes)));
     }
     const int npad = tc_npad(p.N);
-    dim3 grid((p.M + C::BM - 1) / C::BM, (p.N + BN - 1) / BN);
+    const int n_img = MODE == LD_HALO ? p.M / (p.OH * p.OW) : 0;
+    dim3 grid(MODE == LD_HALO ? n_img * halo_tiles_per_img(p) : (p.M + C::BM - 1) / C::BM, (p.N + BN - 1) / BN);
     // Split-K over a thread-block cluster for long reductions on under-filled grids (the K loop is the serial part of
     // these latency-bound launches): 4 or 2 CTAs per output tile, each >= 4 chunks, at most ~one wave of CTAs.
+    // LD_HALO splits by whole channel chunks, into at most one wave of the 132 SMs (layer2 at one pair: 72 tiles split
+    // by 2 measured 23.4 us against 17.3 us for the im2col launch, its 12 CTAs past the wave running on their own; H100 at 400 W).
     int ksplit = 1;
     if constexpr (!LN && BN <= 64 && MODE != LD_STEM4) {
         const int kc = (p.K + BK - 1) / BK;
+        const int cc = MODE == LD_HALO ? p.C / BK : kc;
         const long long ctas = (long long)grid.x * grid.y;
+        const long long wave = MODE == LD_HALO ? kNumSms : kWaveCtas;
         if (!(g_tc_variant & 512) && kc >= (16 >> ((g_tc_variant >> 14) & 3))) {     // bring-up knob: bits 14-15
-            if (C::kMaxSplit >= 4 && kc % 4 == 0 && ctas * 4 <= kWaveCtas) ksplit = 4;
-            else if (C::kMaxSplit >= 2 && kc % 2 == 0 && ctas * 2 <= kWaveCtas) ksplit = 2;
+            if (C::kMaxSplit >= 4 && kc % 4 == 0 && cc % 4 == 0 && ctas * 4 <= wave) ksplit = 4;
+            else if (C::kMaxSplit >= 2 && kc % 2 == 0 && cc % 2 == 0 && ctas * 2 <= wave) ksplit = 2;
         }
+    }
+    if constexpr (MODE == LD_HALO) {
+        // The implicit im2col runs the launch when the halo tiles of a CTA's channel chunks do not fit their region, or
+        // when the halo grid would leave a third of the SMs idle (layer2 at one pair: 72 CTAs of 18 chunks measured
+        // 19.0 us against 17.3 us for the 128 im2col CTAs of 9 chunks; layer3's 96 halo CTAs beat its im2col grid).
+        const int ccp = p.C / BK / ksplit;
+        if (ccp > kHaloMaxChunks || (uint32_t)ccp * 2u * halo_plane_bytes(p) > kHaloMaxBytes ||
+            (long long)grid.x * grid.y * ksplit < kHaloMinCtas)
+            return launch_one<BN, LN, LD_CONV>(p, s);
+        COTR_CHECK(p.M == n_img * p.OH * p.OW && p.res.hi == nullptr && p.addmat == nullptr && !p.remap && p.out_f32 == nullptr,
+                   "gemm_tc: the halo loader needs whole images and a plain split16 output");
     }
     COTR_CHECK(p.a_ln_cs == nullptr || (DLN && p.K == 256 && p.a_mode == A_ROWMAJOR && p.a_ln_part != nullptr),
                "gemm_tc: the deferred LayerNorm on A needs a row-major operand with K = 256 and its partial statistics");
@@ -711,6 +812,13 @@ int launch_one(const GemmParams& p, cudaStream_t s) {
     const size_t smem = C::kSmemBytes + (size_t)(ksplit - 1) * (C::BM / ksplit) * C::kPartPitch;     // incoming partial rows
     COTR_CHECK_CUDA(launch_kernel_cluster(gemm_tc_kernel<BN, LN, MODE, DLN>, grid, dim3(kThreads), smem, s, ksplit, p, npad));
     return 0;
+}
+
+// 3x3 stride-1 "same" convolutions over whole images take the halo loader; cotr_debug_set_variant bit 20 keeps them on
+// the implicit im2col (an in-process A/B and the reference of tests/test_conv_halo_gpu.py)
+inline bool halo_conv(const GemmParams& p) {
+    return p.a_mode == A_CONV_NHWC && p.KH == 3 && p.KW == 3 && p.stride == 1 && p.pad == 1 && p.OH == p.H && p.OW == p.W &&
+           (p.C & 63) == 0 && !(g_tc_variant & (1 << 20));
 }
 
 template <int BN, bool LN>
@@ -724,7 +832,10 @@ int launch_mode(const GemmParams& p, cudaStream_t s) {
         return launch_one<BN, LN, LD_GATHER>(p, s);
     }
     if constexpr (!LN && BN >= 32) {
-        if (p.a_mode == A_CONV_NHWC && (p.C & 63) == 0) return launch_one<BN, LN, LD_CONV>(p, s);
+        if (p.a_mode == A_CONV_NHWC && (p.C & 63) == 0) {
+            if (halo_conv(p)) return launch_one<BN, LN, LD_HALO>(p, s);
+            return launch_one<BN, LN, LD_CONV>(p, s);
+        }
     }
     if constexpr (!LN && BN == 64) {
         if (p.a_mode == A_STEM_NHWC4 && p.K == kStemK) return launch_one<64, false, LD_STEM4>(p, s);
@@ -829,7 +940,7 @@ int launch_gemm_tc(const GemmParams& p, cudaStream_t s) {
     // 128 x 128 register accumulator leaves room for a single main slot, and the longer truncating chain of the
     // K = 1152 / 2304 convolutions then moved the 16-pair fixture's predictions 3.7e-4 from the fp64 reference (H100)
     // where the 64-wide tile's two main slots keep it within the 3e-4 the tests hold it to.
-    const long long mt = (p.M + 127) / 128;
+    const long long mt = halo_conv(p) ? (long long)(p.M / (p.OH * p.OW)) * halo_tiles_per_img(p) : (p.M + 127) / 128;
     // bring-up knob (cotr_debug_set_variant): bits 10-11 move the CTA-count threshold of the 64-wide tile
     static const long long kThr[4] = {86, 43, 57, 132};
     const long long thr64 = kThr[(g_tc_variant >> 10) & 3];

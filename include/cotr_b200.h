@@ -241,7 +241,8 @@ int cotr_test_attention_weights(int path, const float* q_dev, const float* k_dev
  * minimum K of split-K (16 >> n chunks of 64).  Schedule: by default a transformer section with >= 2048 rows runs the
  * deferred-LayerNorm schedule (no LayerNorm launches), smaller ones the explicit one, in which each feed-forward block
  * (linear1, linear2, its LayerNorm) is one fused launch on the tensor-core path; bit 19 forces deferred everywhere,
- * bit 16 never and runs every feed-forward block as separate linear1 / linear2 / LayerNorm launches.
+ * bit 16 never and runs every feed-forward block as separate linear1 / linear2 / LayerNorm launches.  Bit 20 (1048576)
+ * runs the 3x3 stride-1 convolutions on the implicit-im2col loader instead of the halo loader (same launches).
  * Process-wide; graphs captured under another value are NOT dropped (call cotr_set_gemm_path twice to drop them). */
 void cotr_debug_set_variant(int variant);
 
