@@ -45,6 +45,9 @@ _PROTOTYPES = {
                                                      ctypes.c_void_p, ctypes.c_void_p]),
     "cotr_decode_attention": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int,
                                              ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]),
+    "cotr_encode_images": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p]),
+    "cotr_encode_context_pairs": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p, ctypes.c_int,
+                                                 ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p]),
     "cotr_forward": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p]),
     "cotr_forward_host": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_void_p]),
     "cotr_preprocess": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_void_p, ctypes.c_int,
@@ -191,6 +194,30 @@ class NativeModel:
         attn = torch.empty((bin(layer_mask).count("1"), B, 512, 512), dtype=torch.float32, device=img.device)
         check(lib().cotr_encode_context_attention(self.handle, _ptr(img), B, ctx.handle, int(layer_mask),
                                                   _ptr(attn) if layer_mask else None, self._stream()), "cotr_encode_context_attention")
+        ctx.pairs = B
+        return attn
+
+    def encode_images(self, images):
+        """(N,3,256,256) fp32 device images -> their backbone features, a (2, N, 256, 1024) float16 device tensor
+        (plane, image, 16x16 position, channel: COTR_IMAGE_FEATURE_BYTES per image) (cotr_encode_images)."""
+        N = images.shape[0]
+        feat = torch.empty((2, N, 256, 1024), dtype=torch.float16, device=images.device)
+        check(lib().cotr_encode_images(self.handle, _ptr(images), N, _ptr(feat), self._stream()), "cotr_encode_images")
+        return feat
+
+    def encode_context_pairs(self, feat, pairs, ctx):
+        """Encode the pairs (B,2) of images of `feat` (from encode_images) into ctx (cotr_encode_context_pairs)."""
+        self.encode_context_pairs_attention(feat, pairs, ctx, 0)
+
+    def encode_context_pairs_attention(self, feat, pairs, ctx, layer_mask):
+        """encode_context_pairs that also returns the encoder attention maps selected by `layer_mask`, as
+        encode_context_attention does: (popcount(layer_mask), B, 512, 512) fp32."""
+        pairs = np.ascontiguousarray(pairs, dtype=np.int32)
+        B = pairs.shape[0]
+        attn = torch.empty((bin(layer_mask).count("1"), B, 512, 512), dtype=torch.float32, device=feat.device)
+        check(lib().cotr_encode_context_pairs(self.handle, _ptr(feat), feat.shape[1], ctypes.c_void_p(pairs.ctypes.data), B,
+                                              ctx.handle, int(layer_mask), _ptr(attn) if layer_mask else None, self._stream()),
+              "cotr_encode_context_pairs")
         ctx.pairs = B
         return attn
 

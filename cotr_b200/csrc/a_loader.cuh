@@ -23,7 +23,7 @@ __device__ __forceinline__ ARow decode_a_row(const GemmParams& p, int m) {
     } else if (p.a_mode == A_TOKENS) {
         // backbone.py:85 concatenates the two halves along W; transformer.py:50 flattens (i, j) -> i*32 + j
         const int pair = m >> 9, t = m & 511, i = t >> 5, j = t & 31;
-        const int row = ((2 * pair + (j >> 4)) * 16 + i) * 16 + (j & 15);
+        const int row = (p.a_pairs[2 * pair + (j >> 4)] * 16 + i) * 16 + (j & 15);
         r.off = (size_t)row * p.lda;
     } else {
         const int ohw = p.OH * p.OW;

@@ -152,7 +152,7 @@ enum AMode : int {
     A_ROWMAJOR = 0,   // A[m * lda + k]
     A_CONV_NHWC = 1,  // implicit im2col over an NHWC activation: m -> (n, oh, ow), k -> (kh, kw, c)
     A_STEM_NHWC4 = 2, // 7x7 stride-2 stem: implicit im2col over the zero-bordered split16 NHWC4 copy of the canvas (below)
-    A_TOKENS = 3,     // m = pair*512 + i*32 + j gathers row ((2*pair + (j>>4))*16 + i)*16 + (j&15)
+    A_TOKENS = 3,     // m = pair*512 + i*32 + j gathers row ((a_pairs[2*pair + (j>>4)])*16 + i)*16 + (j&15)
 };
 
 // D[M,N] = epilogue( A[M,K] * W[N,K]^T ).
@@ -162,6 +162,9 @@ struct GemmParams {
     CSplit16 a;
     int a_mode;
     int lda;
+    // A_TOKENS: [pairs][2] device table, the (left, right) image of each pair among the (n,16,16,1024) images of `a`.
+    // Written before the launch by a copy, never by a kernel, so the loaders may read it before the dependency wait.
+    const int* a_pairs;
     int H, W, C;      // convolution geometry: input height / width / channels (per image)
     int OH, OW;       // output height / width
     int KH, KW, stride, pad;
@@ -273,8 +276,9 @@ int launch_layernorm(CSplit16 x, const float* gamma, const float* beta, Split16 
 int launch_ln_partials(CSplit16 x, float2* part, int rows, cudaStream_t s);
 int launch_layernorm_twice(CSplit16 x, const float* g1, const float* b1, const float* g2, const float* b2, Split16 out, int rows, cudaStream_t s);
 int launch_query_encode(const float* queries, Split16 qpos, int rows, cudaStream_t s);
-// fp32 (B,3,256,512) canvas -> the stem's bordered split16 NHWC4 operand (2B images of kStemCanvasElems halves per plane)
-int launch_stem_canvas(const float* img, Split16 canvas, int n_img, cudaStream_t s);
+// n_img fp32 256x256 images -> the stem's bordered split16 NHWC4 operand (kStemCanvasElems halves per image and plane).
+// halves: img is a (n_img/2,3,256,512) canvas, image n = 2*pair + half; otherwise a (n_img,3,256,256) batch.
+int launch_stem_canvas(const float* img, bool halves, Split16 canvas, int n_img, cudaStream_t s);
 int launch_f32_to_split16(const float* in, Split16 out, size_t n, cudaStream_t s);
 int launch_split16_to_f32(CSplit16 in, float* out, size_t n, cudaStream_t s);
 

@@ -40,16 +40,21 @@ __global__ void maxpool_3x3s2_nhwc_kernel(const CSplit16 in, const Split16 out, 
     }
 }
 
-// The stem's operand (common.cuh "The stem's input"): fp32 (B,3,256,512) NCHW canvas -> per image n = 2*pair + half the
-// split16 NHWC4 copy with a zero border.  One thread per pixel: three coalesced channel reads, one 8-byte store per plane.
-__global__ void __launch_bounds__(256) stem_canvas_kernel(const float* __restrict__ img, const Split16 canvas, int n_img) {
+// The stem's operand (common.cuh "The stem's input"): fp32 NCHW 256x256 images -> per image n the split16 NHWC4 copy with
+// a zero border.  Image n starts at img + (n >> 1) * pair_stride + (n & 1) * half_offset and has row pitch `pitch` (channel
+// stride 256 * pitch), which covers both sources: the halves of a (B,3,256,512) canvas (3*256*512, 256, 512) and a
+// (N,3,256,256) batch (2*3*256*256, 3*256*256, 256).  One thread per pixel: three coalesced channel reads, one 8-byte
+// store per plane.
+__global__ void __launch_bounds__(256) stem_canvas_kernel(const float* __restrict__ img, size_t pair_stride, size_t half_offset,
+                                                          int pitch, const Split16 canvas, int n_img) {
     if (threadIdx.x == 0) pdl_launch_dependents();
     pdl_wait();
     const size_t total = (size_t)n_img * 256 * 256;
+    const size_t plane = (size_t)256 * pitch;
     for (size_t idx = blockIdx.x * (size_t)blockDim.x + threadIdx.x; idx < total; idx += (size_t)gridDim.x * blockDim.x) {
         const int x = (int)(idx & 255), y = (int)((idx >> 8) & 255), n = (int)(idx >> 16);
-        const float* src = img + (size_t)(n >> 1) * 3 * 256 * 512 + (size_t)y * 512 + (n & 1) * 256 + x;
-        const float r = __ldcg(src), g = __ldcg(src + 256 * 512), b = __ldcg(src + 2 * 256 * 512);
+        const float* src = img + (size_t)(n >> 1) * pair_stride + (n & 1) * half_offset + (size_t)y * pitch + x;
+        const float r = __ldcg(src), g = __ldcg(src + plane), b = __ldcg(src + 2 * plane);
         uint2 h, l;
         split_f16x2(r, g, h.x, l.x);
         split_f16x2(b, 0.f, h.y, l.y);
@@ -212,9 +217,13 @@ int launch_query_encode(const float* queries, Split16 qpos, int rows, cudaStream
     return 0;
 }
 
-int launch_stem_canvas(const float* img, Split16 canvas, int n_img, cudaStream_t s) {
+int launch_stem_canvas(const float* img, bool halves, Split16 canvas, int n_img, cudaStream_t s) {
     if (n_img <= 0) return 0;
-    COTR_CHECK_CUDA(launch_kernel(stem_canvas_kernel, dim3(grid_for((size_t)n_img * 256 * 256, 256)), dim3(256), 0, s, img, canvas, n_img));
+    const size_t img_elems = (size_t)3 * 256 * 256;
+    const size_t pair_stride = 2 * img_elems, half_offset = halves ? 256 : img_elems;
+    const int pitch = halves ? 512 : 256;
+    COTR_CHECK_CUDA(launch_kernel(stem_canvas_kernel, dim3(grid_for((size_t)n_img * 256 * 256, 256)), dim3(256), 0, s, img, pair_stride,
+                                  half_offset, pitch, canvas, n_img));
     return 0;
 }
 

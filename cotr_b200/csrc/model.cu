@@ -83,6 +83,7 @@ struct Workspace {
     Split16 canvas = kNoSplit, stem = kNoSplit, bx = kNoSplit, by = kNoSplit, bt1 = kNoSplit, bt2 = kNoSplit, bds = kNoSplit;
     // encoder
     Split16 src = kNoSplit, xa = kNoSplit, xb = kNoSplit, qk = kNoSplit, vt = kNoSplit, ao = kNoSplit, ffh = kNoSplit;
+    int* pair_id = nullptr;              // [pairs][2] = (2p, 2p+1): input_proj's image table for canvases (constant, graph-safe)
     unsigned char* kvimg = nullptr;      // [pairs][8 heads] attention operand images of the encoder's own k / v
     float* ln_tmp = nullptr;      // fp32 [tokens][256]: pre-LayerNorm rows of the SIMT cross-check path
     float2 *enc_st_a = nullptr, *enc_st_b = nullptr;     // [tokens][16] partial row statistics of xa / xb (deferred LayerNorms)
@@ -139,6 +140,12 @@ struct cotr_model {
     std::map<long long, cudaGraphExec_t> graphs;
     std::map<long long, int> graph_launches;
     std::set<long long> shapes_seen;
+    // cotr_encode_context_pairs: the caller's (B,2) image table, staged through pinned memory.  pair_copied is recorded
+    // after each copy out of pair_stage; the host rewrites pair_stage only once that copy has completed.
+    int* pair_tab = nullptr;
+    int* pair_stage = nullptr;
+    int pair_cap = 0;
+    cudaEvent_t pair_copied = nullptr;
     cotr::Preprocessor* pre = nullptr;         // device-side crop / resize / normalise (cotr_preprocess)
     cotr::FlowMerger* merger = nullptr;        // device-side tail of the dense first guess (cotr_flow_tile_merge)
     bool prof_on = false;
@@ -566,6 +573,7 @@ int ensure_encode_ws(cotr_model* m, int B) {
     if (B <= w.cap_pairs) return 0;
     COTR_CHECK_CUDA(cudaDeviceSynchronize());
     drop_graphs(m);
+    w.cap_pairs = 0;      // a failed allocation below leaves no capacity behind, so the next call allocates again
     Split16* bufs[] = {&w.canvas, &w.stem, &w.bx, &w.by, &w.bt1, &w.bt2, &w.bds, &w.src, &w.xa, &w.xb, &w.qk, &w.vt, &w.ao, &w.ffh};
     for (Split16* b : bufs) ws_free(b);
     ws_free_f32(&w.ln_tmp);
@@ -580,6 +588,11 @@ int ensure_encode_ws(cotr_model* m, int B) {
         ws_alloc(&w.ffh, tok * kFF) || ws_alloc_f32(&w.ln_tmp, tok * kDModel) ||
         ws_alloc_f32(reinterpret_cast<float**>(&w.enc_st_a), tok * 32) || ws_alloc_f32(reinterpret_cast<float**>(&w.enc_st_b), tok * 32))
         return 1;
+    if (w.pair_id) { cudaFree(w.pair_id); w.pair_id = nullptr; }
+    std::vector<int> ident(2 * (size_t)B);
+    for (size_t i = 0; i < ident.size(); ++i) ident[i] = (int)i;
+    COTR_CHECK_CUDA(cudaMalloc((void**)&w.pair_id, ident.size() * sizeof(int)));
+    COTR_CHECK_CUDA(cudaMemcpy(w.pair_id, ident.data(), ident.size() * sizeof(int), cudaMemcpyHostToDevice));
     COTR_CHECK_CUDA(cudaMalloc((void**)&w.kvimg, (size_t)B * kHeads * kAttnHeadImgBytes));
     // the 16 pad bytes of every value key group are copied by the bulk TMA: keep them defined
     COTR_CHECK_CUDA(cudaMemset(w.kvimg, 0, (size_t)B * kHeads * kAttnHeadImgBytes));
@@ -594,6 +607,7 @@ int ensure_decode_ws(cotr_model* m, int rows) {
     if (rows <= w.cap_rows) return 0;
     COTR_CHECK_CUDA(cudaDeviceSynchronize());
     drop_graphs(m);
+    w.cap_rows = 0;       // as in ensure_encode_ws: no stale capacity after a failed allocation
     Split16* bufs[] = {&w.qpos, &w.qp, &w.t, &w.qb, &w.dao, &w.dh, &w.hs, &w.hd1, &w.hd2, &w.t2};
     for (Split16* b : bufs) ws_free(b);
     ws_free_f32(&w.dln_tmp);
@@ -613,22 +627,18 @@ int ensure_decode_ws(cotr_model* m, int rows) {
 // ----------------------------------------------------------------------------------------------
 // forward schedule
 // ----------------------------------------------------------------------------------------------
-int encode_impl(cotr_model* m, const float* img, int B, cotr_context* ctx, cudaStream_t s, const AttnMaps& maps = AttnMaps()) {
-    COTR_CHECK(B >= 1, "cotr_encode_context: B must be >= 1 (got %d)", B);
-    COTR_CHECK(ctx && ctx->model == m, "cotr_encode_context: context does not belong to this model");
-    COTR_CHECK(B <= ctx->max_pairs, "cotr_encode_context: B = %d exceeds the context capacity %d", B, ctx->max_pairs);
-    COTR_CHECK_CUDA(cudaSetDevice(m->device));
-    if (ensure_encode_ws(m, B)) return 1;
+// The backbone of n_img 256x256 images (halves: the two halves of n_img/2 canvases, else a (n_img,3,256,256) batch) up to
+// layer3; the last bottleneck writes the (n_img,16,16,1024) NHWC features to `feat`.  The workspace must hold n_img images.
+int encode_backbone(cotr_model* m, const float* img, bool halves, int n_img, Split16 feat, cudaStream_t s) {
     Workspace& w = m->ws;
     Run r{m, s};
-    const int n_img = 2 * B;
     const CSplit16 none{nullptr, nullptr};
 
     // backbone.py:81-82: the two 256x256 halves go through the ResNet body as independent images.
     // Stem: conv 7x7/2 (+FrozenBN folded) + ReLU, then MaxPool 3x3/2  (torchvision resnet.py _forward_impl).
     {
         LaunchScope scope(r, K_STEM_CANVAS, n_img * 256 * 256, 4, 0);
-        if (launch_stem_canvas(img, w.canvas, n_img, s)) return 1;
+        if (launch_stem_canvas(img, halves, w.canvas, n_img, s)) return 1;
     }
     if (run_conv(r, m->stem, n_img, cs(w.canvas), 256, 256, w.stem, true, none)) return 1;
     {
@@ -639,7 +649,8 @@ int encode_impl(cotr_model* m, const float* img, int B, cotr_context* ctx, cudaS
     Split16 x = w.bx;
     Split16 y = w.by;
     int H = 64, W = 64;
-    for (const Block& b : m->blocks) {
+    for (size_t i = 0; i < m->blocks.size(); ++i) {
+        const Block& b = m->blocks[i];
         // torchvision Bottleneck (v1.5): 1x1 -> 3x3(stride) -> 1x1, + identity | downsample, ReLU
         if (run_conv(r, b.c1, n_img, cs(x), H, W, w.bt1, true, none)) return 1;
         if (run_conv(r, b.c2, n_img, cs(w.bt1), H, W, w.bt2, true, none)) return 1;
@@ -649,18 +660,27 @@ int encode_impl(cotr_model* m, const float* img, int B, cotr_context* ctx, cudaS
             if (run_conv(r, b.ds, n_img, cs(x), H, W, w.bds, false, none)) return 1;
             identity = cs(w.bds);
         }
+        if (i + 1 == m->blocks.size()) y = feat;
         if (run_conv(r, b.c3, n_img, cs(w.bt2), OH, OW, y, true, identity)) return 1;
         Split16 t = x; x = y; y = t;
         H = OH; W = OW;
     }
-    m->last_feat = x;   // (2B,16,16,1024) NHWC
+    return 0;
+}
+
+// Everything of the context after the backbone, for B pairs: pair p is the canvas [image pairs[2p] | image pairs[2p+1]]
+// of the (n,16,16,1024) NHWC features `feat` (pairs: [B][2] device table, see GemmParams::a_pairs).
+int encode_tail(cotr_model* m, CSplit16 feat, const int* pairs, int B, cotr_context* ctx, cudaStream_t s, const AttnMaps& maps) {
+    Workspace& w = m->ws;
+    Run r{m, s};
 
     // cotr_model.py:37 input_proj (1x1 conv 1024 -> 256) fused with the left|right concat (backbone.py:85)
     // and the flatten to token-major (transformer.py:50): row = pair*512 + i*32 + j.
     const int T = B * kTokens;
     {
-        GemmParams p = gemm_base(T, kDModel, 1024, cs(x), 1024, m->proj.w, m->proj.wtc, m->proj.wtc_scale, w.src, kDModel);
+        GemmParams p = gemm_base(T, kDModel, 1024, feat, 1024, m->proj.w, m->proj.wtc, m->proj.wtc_scale, w.src, kDModel);
         p.a_mode = A_TOKENS;
+        p.a_pairs = pairs;
         p.bias = m->proj.b;
         if (run_gemm(r, p, nullptr)) return 1;
     }
@@ -785,6 +805,61 @@ int encode_impl(cotr_model* m, const float* img, int B, cotr_context* ctx, cudaS
     ctx->holds_img = tc;
     m->last_pairs = B;
     return 0;
+}
+
+int check_context(cotr_model* m, const char* fn, int B, const cotr_context* ctx) {
+    COTR_CHECK(B >= 1, "%s: B must be >= 1 (got %d)", fn, B);
+    COTR_CHECK(ctx && ctx->model == m, "%s: context does not belong to this model", fn);
+    COTR_CHECK(B <= ctx->max_pairs, "%s: B = %d exceeds the context capacity %d", fn, B, ctx->max_pairs);
+    return 0;
+}
+
+int encode_impl(cotr_model* m, const float* img, int B, cotr_context* ctx, cudaStream_t s, const AttnMaps& maps = AttnMaps()) {
+    if (check_context(m, "cotr_encode_context", B, ctx)) return 1;
+    COTR_CHECK_CUDA(cudaSetDevice(m->device));
+    if (ensure_encode_ws(m, B)) return 1;
+    Workspace& w = m->ws;
+    if (encode_backbone(m, img, true, 2 * B, w.bx, s)) return 1;
+    m->last_feat = w.bx;   // (2B,16,16,1024) NHWC
+    return encode_tail(m, cs(w.bx), w.pair_id, B, ctx, s, maps);
+}
+
+// Images per backbone pass of cotr_encode_images: the backbone workspace of a 32-pair context.
+constexpr int kImageChunk = 64;
+constexpr size_t kFeatElems = 16 * 16 * 1024;     // per image and plane (COTR_IMAGE_FEATURE_BYTES / 4)
+
+int encode_images_impl(cotr_model* m, const float* img, int N, void* feat_dev, cudaStream_t s) {
+    if (ensure_encode_ws(m, (std::min(N, kImageChunk) + 1) / 2)) return 1;
+    __half* hi = static_cast<__half*>(feat_dev);
+    __half* lo = hi + (size_t)N * kFeatElems;
+    for (int n0 = 0; n0 < N; n0 += kImageChunk) {
+        const int n = std::min(kImageChunk, N - n0);
+        const Split16 dst{hi + (size_t)n0 * kFeatElems, lo + (size_t)n0 * kFeatElems};
+        if (encode_backbone(m, img + (size_t)n0 * 3 * 256 * 256, false, n, dst, s)) return 1;
+    }
+    return 0;
+}
+
+int encode_pairs_impl(cotr_model* m, const void* feat_dev, int n_images, const int32_t* pairs, int B, cotr_context* ctx,
+                      cudaStream_t s, const AttnMaps& maps) {
+    if (ensure_encode_ws(m, B)) return 1;
+    if (B > m->pair_cap) {
+        COTR_CHECK_CUDA(cudaDeviceSynchronize());
+        if (m->pair_tab) { cudaFree(m->pair_tab); m->pair_tab = nullptr; }
+        if (m->pair_stage) { cudaFreeHost(m->pair_stage); m->pair_stage = nullptr; }
+        m->pair_cap = 0;
+        COTR_CHECK_CUDA(cudaMalloc((void**)&m->pair_tab, 2 * (size_t)B * sizeof(int)));
+        COTR_CHECK_CUDA(cudaMallocHost((void**)&m->pair_stage, 2 * (size_t)B * sizeof(int)));
+        m->pair_cap = B;
+    }
+    if (!m->pair_copied) COTR_CHECK_CUDA(cudaEventCreateWithFlags(&m->pair_copied, cudaEventDisableTiming));
+    // the previous call's copy out of the staging buffer has long completed unless the host runs a whole call ahead
+    COTR_CHECK_CUDA(cudaEventSynchronize(m->pair_copied));
+    memcpy(m->pair_stage, pairs, 2 * (size_t)B * sizeof(int));
+    COTR_CHECK_CUDA(cudaMemcpyAsync(m->pair_tab, m->pair_stage, 2 * (size_t)B * sizeof(int), cudaMemcpyHostToDevice, s));
+    COTR_CHECK_CUDA(cudaEventRecord(m->pair_copied, s));
+    const __half* hi = static_cast<const __half*>(feat_dev);
+    return encode_tail(m, CSplit16{hi, hi + (size_t)n_images * kFeatElems}, m->pair_tab, B, ctx, s, maps);
 }
 
 // maps.base: this chunk's first row (pair pair0, its first query) in the caller's (n_sel, B, Q, 512) buffer
@@ -1141,6 +1216,10 @@ void cotr_destroy(cotr_model* m) {
                        &w.qpos, &w.qp, &w.t, &w.qb, &w.dao, &w.dh, &w.hs, &w.hd1, &w.hd2, &w.t2};
     for (Split16* b : bufs) ws_free(b);
     if (w.kvimg) cudaFree(w.kvimg);
+    if (w.pair_id) cudaFree(w.pair_id);
+    if (m->pair_tab) cudaFree(m->pair_tab);
+    if (m->pair_stage) cudaFreeHost(m->pair_stage);
+    if (m->pair_copied) cudaEventDestroy(m->pair_copied);
     float** fbufs[] = {&w.ln_tmp, &w.dln_tmp, &w.img_stage, &w.q_stage, &w.pred_stage,
                        reinterpret_cast<float**>(&w.enc_st_a), reinterpret_cast<float**>(&w.enc_st_b),
                        reinterpret_cast<float**>(&w.dec_st_a), reinterpret_cast<float**>(&w.dec_st_b)};
@@ -1218,6 +1297,40 @@ int cotr_encode_context_attention(cotr_model* m, const float* img_dev, int B, co
     return encode_impl(m, img_dev, B, ctx, (cudaStream_t)cuda_stream, maps);
 }
 
+int cotr_encode_images(cotr_model* m, const float* img_dev, int N, void* feat_dev, void* cuda_stream) {
+    COTR_CHECK(m && img_dev && feat_dev, "cotr_encode_images: null argument");
+    COTR_CHECK(N >= 1, "cotr_encode_images: N must be >= 1 (got %d)", N);
+    COTR_CHECK(((uintptr_t)img_dev & 3) == 0, "cotr_encode_images: img_dev is not 4-byte aligned");
+    COTR_CHECK(((uintptr_t)feat_dev & 15) == 0, "cotr_encode_images: feat_dev is not 16-byte aligned");
+    COTR_CHECK_CUDA(cudaSetDevice(m->device));
+    CallOrder order(m, (cudaStream_t)cuda_stream);
+    m->launches = 0;
+    return encode_images_impl(m, img_dev, N, feat_dev, (cudaStream_t)cuda_stream);
+}
+
+int cotr_encode_context_pairs(cotr_model* m, const void* feat_dev, int n_images, const int32_t* pairs_host, int B,
+                              cotr_context* ctx, int layer_mask, float* attn_dev, void* cuda_stream) {
+    const char* fn = "cotr_encode_context_pairs";
+    COTR_CHECK(m && feat_dev && pairs_host, "%s: null argument", fn);
+    COTR_CHECK(((uintptr_t)feat_dev & 15) == 0, "%s: feat_dev is not 16-byte aligned", fn);
+    COTR_CHECK(((uintptr_t)attn_dev & 3) == 0, "%s: attn_dev is not 4-byte aligned", fn);
+    COTR_CHECK(n_images >= 1, "%s: n_images must be >= 1 (got %d)", fn, n_images);
+    if (check_context(m, fn, B, ctx)) return 1;
+    for (int i = 0; i < 2 * B; ++i)
+        COTR_CHECK(pairs_host[i] >= 0 && pairs_host[i] < n_images, "%s: pairs[%d][%d] = %d is outside [0, %d)", fn, i / 2, i % 2,
+                   (int)pairs_host[i], n_images);
+    if (check_layer_mask(fn, layer_mask, attn_dev, kEncLayers)) return 1;
+    COTR_CHECK_CUDA(cudaSetDevice(m->device));
+    CallOrder order(m, (cudaStream_t)cuda_stream);
+    m->launches = 0;
+    AttnMaps maps;
+    maps.mask = (unsigned)layer_mask;
+    maps.base = attn_dev;
+    maps.layer_stride = (size_t)B * kTokens * kTokens;
+    maps.pair_stride = (size_t)kTokens * kTokens;
+    return encode_pairs_impl(m, feat_dev, n_images, pairs_host, B, ctx, (cudaStream_t)cuda_stream, maps);
+}
+
 int cotr_decode_attention(cotr_model* m, const cotr_context* ctx, const float* queries_dev, int B, int Q, int layer_mask,
                           float* attn_dev, float* pred_dev, void* cuda_stream) {
     COTR_CHECK(m && (Q == 0 || (queries_dev && pred_dev)), "cotr_decode_attention: null argument");
@@ -1243,6 +1356,7 @@ int ensure_stage(cotr_model* m, int B, int Q) {
         COTR_CHECK_CUDA(cudaDeviceSynchronize());
         drop_graphs(m);
         ws_free_f32(&w.img_stage);
+        w.img_stage_elems = 0;
         if (ws_alloc_f32(&w.img_stage, img_elems)) return 1;
         w.img_stage_elems = img_elems;
     }
@@ -1250,6 +1364,7 @@ int ensure_stage(cotr_model* m, int B, int Q) {
         COTR_CHECK_CUDA(cudaDeviceSynchronize());
         drop_graphs(m);
         ws_free_f32(&w.q_stage); ws_free_f32(&w.pred_stage);
+        w.q_stage_elems = 0;
         if (ws_alloc_f32(&w.q_stage, q_elems ? q_elems : 2) || ws_alloc_f32(&w.pred_stage, q_elems ? q_elems : 2)) return 1;
         w.q_stage_elems = q_elems;
     }
@@ -1533,7 +1648,7 @@ int cotr_test_gemm(const cotr_test_gemm_desc* d, const float* A_dev, const float
         const int n_img = d->M / (128 * 128);
         if (a16.empty((size_t)n_img * kStemCanvasElems)) return 1;
         COTR_CHECK_CUDA(cudaMemset(a16.t.hi, 0, (size_t)n_img * kStemCanvasElems * 2 * sizeof(__half)));
-        if (launch_stem_canvas(A_dev, a16.t, n_img, 0)) return 1;
+        if (launch_stem_canvas(A_dev, true, a16.t, n_img, 0)) return 1;
         p.a = cs(a16.t);
         w_stem = stem_weight_order(std::vector<float>(w_host, w_host + (size_t)d->N * 147), d->N);
         w_host = w_stem.data();
@@ -1542,6 +1657,14 @@ int cotr_test_gemm(const cotr_test_gemm_desc* d, const float* A_dev, const float
         COTR_CHECK(d->a_elems > 0, "cotr_test_gemm: a_elems missing");
         if (a16.from_f32(A_dev, (size_t)d->a_elems)) return 1;
         p.a = cs(a16.t);
+    }
+    int* pair_id = nullptr;
+    if (d->a_mode == A_TOKENS) {            // the canvas order, as cotr_encode_context runs it: pair p = images (2p, 2p+1)
+        std::vector<int> ident(2 * (size_t)((d->M + kTokens - 1) / kTokens));
+        for (size_t i = 0; i < ident.size(); ++i) ident[i] = (int)i;
+        COTR_CHECK_CUDA(cudaMalloc((void**)&pair_id, ident.size() * sizeof(int)));
+        COTR_CHECK_CUDA(cudaMemcpy(pair_id, ident.data(), ident.size() * sizeof(int), cudaMemcpyHostToDevice));
+        p.a_pairs = pair_id;
     }
     if (residual_dev) {
         if (res16.from_f32(residual_dev, (size_t)d->M * d->ldr)) return 1;
@@ -1628,6 +1751,7 @@ int cotr_test_gemm(const cotr_test_gemm_desc* d, const float* A_dev, const float
     if (cb_dev) cudaFree(cb_dev);
     if (stats_dev) cudaFree(stats_dev);
     if (res_stats_dev) cudaFree(res_stats_dev);
+    if (pair_id) cudaFree(pair_id);
     if (rc) return rc;
     COTR_CHECK(e == cudaSuccess, "cotr_test_gemm: kernel failed: %s", cudaGetErrorString(e));
     return 0;

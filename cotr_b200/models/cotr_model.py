@@ -26,8 +26,10 @@ decoder hooks, so a caller that encodes once and decodes twice (cotr_corr_base's
 fire once where the reference fires them twice.  Without hooks nothing of this runs.  Forward pre-hooks and the
 sharded model are not covered.
 """
+import itertools
 import math
 
+import numpy as np
 import torch
 from torch import nn
 
@@ -155,6 +157,20 @@ class Context:
         self.batch = batch
 
 
+class ImageFeatures:
+    """Backbone features of N 256x256 images (see cotr_encode_images): `tensor` is (2, N, 256, 1024) float16 on the
+    device, the layer3 output in the library's split16 storage (hi and lo planes; the value is hi + lo).  They belong to
+    the weights of the model that made them: `generation` changes whenever that model's weights are repacked."""
+
+    def __init__(self, tensor, n, generation):
+        self.tensor = tensor
+        self.n = n
+        self.generation = generation
+
+
+_generations = itertools.count(1)      # process-wide, so that features never match another model's weights
+
+
 class COTR(nn.Module):
     def __init__(self, args=None):
         super().__init__()
@@ -185,9 +201,11 @@ class COTR(nn.Module):
         self._native = None
         self._ctx_cache = {}
         self._hook_ctx = None                     # context of hooked forwards (grown to the largest batch seen)
+        self._generation = next(_generations)     # the weights ImageFeatures were made with
 
     # ---- native handle management ---------------------------------------------------------------------
     def _invalidate(self):
+        self._generation = next(_generations)
         for ctx in self._ctx_cache.values():
             ctx.close()
         self._ctx_cache = {}
@@ -324,24 +342,64 @@ class COTR(nn.Module):
         (inference_helper.py:155-160, :61-75): see cotr_flow_tile_merge in include/cotr_b200.h."""
         self.native().flow_tile_merge(tile, affine, patch, flow, conf, first)
 
-    @torch.no_grad()
-    def encode_context(self, samples, reuse=False):
-        x = self._canvas(samples)
+    def _context(self, batch, reuse):
         nat = self.native()
         if reuse:
             # one cached device K/V buffer per batch size: no cudaMalloc / device-synchronising cudaFree per call.
             # The returned Context is only valid until the next encode_context(reuse=True) of the same batch size.
-            native_ctx = self._ctx_cache.get(x.shape[0])
+            native_ctx = self._ctx_cache.get(batch)
             if native_ctx is None:
                 if len(self._ctx_cache) >= 4:
                     for old in self._ctx_cache.values():
                         old.close()
                     self._ctx_cache = {}
-                native_ctx = self._ctx_cache[x.shape[0]] = capi.NativeContext(nat, x.shape[0])
+                native_ctx = self._ctx_cache[batch] = capi.NativeContext(nat, batch)
         else:
-            native_ctx = capi.NativeContext(nat, x.shape[0])
-        ctx = Context(native_ctx, x.shape[0])
+            native_ctx = capi.NativeContext(nat, batch)
+        return Context(native_ctx, batch)
+
+    @torch.no_grad()
+    def encode_context(self, samples, reuse=False):
+        x = self._canvas(samples)
+        ctx = self._context(x.shape[0], reuse)
         self._encode(x, ctx.native)
+        return ctx
+
+    @torch.no_grad()
+    def encode_images(self, images):
+        """Backbone features of (N,3,256,256) images, each normalised like one half of a canvas (cotr_encode_images).
+        Encode a whole image set in one call: the library runs the backbone 64 images at a time."""
+        assert isinstance(images, torch.Tensor) and images.ndim == 4 and tuple(images.shape[1:]) == (3, MAX_SIZE, MAX_SIZE), \
+            f"images must be (N,3,256,256), got {tuple(getattr(images, 'shape', ()))}"
+        dev = next(self.parameters()).device
+        x = images.to(device=dev, dtype=torch.float32).contiguous()
+        return ImageFeatures(self.native().encode_images(x), x.shape[0], self._generation)
+
+    @torch.no_grad()
+    def encode_context_pairs(self, features, pairs, reuse=False):
+        """The Context of the canvases [image pairs[p][0] | image pairs[p][1]] from cached ImageFeatures; `pairs` is a
+        (B,2) integer tensor, array or list.  `reuse` and the encoder attention hooks work as in encode_context."""
+        if features.generation != self._generation:
+            raise RuntimeError("encode_context_pairs: these ImageFeatures were made with other weights "
+                               "(load_state_dict / .to() / refresh_native since): encode the images again")
+        t = features.tensor
+        dev = next(self.parameters()).device
+        assert t.device == dev and t.dtype == torch.float16 and t.is_contiguous() and tuple(t.shape) == (2, features.n, 256, 1024), \
+            f"features.tensor must be a contiguous (2,{features.n},256,1024) float16 tensor on {dev}"
+        p = pairs.detach().cpu().numpy() if isinstance(pairs, torch.Tensor) else np.asarray(pairs)
+        assert p.ndim == 2 and p.shape[1] == 2 and p.shape[0] >= 1 and p.dtype.kind in "iu", \
+            f"pairs must be a non-empty (B,2) integer table, got shape {p.shape} dtype {p.dtype}"
+        p32 = p.astype(np.int32)
+        if not np.array_equal(p32, p):
+            raise RuntimeError(f"encode_context_pairs: image index outside [0, {features.n})")
+        ctx = self._context(p32.shape[0], reuse)
+        nat = self.native()
+        enc, _ = self._attention_modules()
+        mask = self._hooked(enc)
+        if not mask:
+            nat.encode_context_pairs(features.tensor, p32, ctx.native)
+        else:
+            self._fire(enc, mask, nat.encode_context_pairs_attention(features.tensor, p32, ctx.native, mask))
         return ctx
 
     @torch.no_grad()

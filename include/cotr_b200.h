@@ -89,6 +89,34 @@ int cotr_encode_context_attention(cotr_model* m, const float* img_dev, int B, co
 int cotr_decode_attention(cotr_model* m, const cotr_context* ctx, const float* queries_dev, int B, int Q, int layer_mask,
                           float* attn_dev, float* pred_dev, void* cuda_stream);
 
+/* ---- image-level feature cache ------------------------------------------------------------------------------------
+ * cotr_encode_context runs the backbone over both halves of every canvas, then builds the pair context from the two
+ * feature maps.  An image that takes part in many pairs (one query against a database, all ordered pairs of an image
+ * set, (a|b) and (b|a)) can go through the backbone once: cotr_encode_images caches its features, and
+ * cotr_encode_context_pairs builds contexts from any pairs of cached images.  A context of the pairs (2p, 2p+1) of the
+ * halves of B canvases is bitwise the cotr_encode_context of those canvases, and the two calls launch exactly the
+ * kernels cotr_encode_context launches (for up to 32 pairs).  Both calls run eagerly (no CUDA-graph capture). */
+
+/* Backbone features of one 256x256 image (backbone.py:81-82: each half of a canvas goes through the ResNet body on its own):
+ * the layer3 output in the library's split16 storage, plane-major [hi|lo][N][16][16][1024] fp16 = 1 MiB per image.
+ * Valid for the weights of the model that made it; the bytes may be copied to the host and back. */
+#define COTR_IMAGE_FEATURE_BYTES (2u * 16u * 16u * 1024u * 2u)
+
+/* img_dev: (N,3,256,256) fp32 NCHW, ImageNet-normalised (one half of a cotr_encode_context canvas); N >= 1.
+ * feat_dev: N * COTR_IMAGE_FEATURE_BYTES, 16-byte aligned.  The images go through the backbone 64 at a time, so the
+ * workspace does not grow with N. */
+int cotr_encode_images(cotr_model* m, const float* img_dev, int N, void* feat_dev, void* cuda_stream);
+
+/* The context of B pairs from cached image features: pair p is the canvas [image pairs_host[2p] | image pairs_host[2p+1]]
+ * (left half = the image whose queries have x < 0.5).  pairs_host: B x 2 int32 HOST array, indices in [0, n_images).
+ * layer_mask / attn_dev as in cotr_encode_context_attention (0 / NULL: no maps).  The table is copied to the device
+ * through a pinned staging buffer, so pairs_host may be reused as soon as the call returns; before it refills that
+ * buffer the call waits for the previous call's copy out of it (only a host running a whole call ahead of the device
+ * waits).  Indices are checked on the host before anything is enqueued.  The context works with
+ * cotr_decode and cotr_decode_attention like one from cotr_encode_context. */
+int cotr_encode_context_pairs(cotr_model* m, const void* feat_dev, int n_images, const int32_t* pairs_host, int B,
+                              cotr_context* ctx, int layer_mask, float* attn_dev, void* cuda_stream);
+
 /* cotr_encode_context + cotr_decode on an internal context. */
 int cotr_forward(cotr_model* m, const float* img_dev, const float* queries_dev, int B, int Q,
                  float* pred_dev, void* cuda_stream);
@@ -201,6 +229,7 @@ int cotr_profile_end(cotr_model* m, cotr_launch_record* out, int max_records);
 /* Test hook: copy an intermediate of the LAST forward to the host.  name is one of
  * "feat" (2B,16,16,1024 NHWC, image n = 2*pair + half), "src" / "mem" (B*512,256 token-major),
  * "hs" (B*Q,256, final decoder LayerNorm output; only valid if B*Q fits in one decode chunk).
+ * "feat" is written by cotr_encode_context only (not by cotr_encode_images / cotr_encode_context_pairs).
  * Returns the element count copied, or -1. */
 int64_t cotr_debug_read(cotr_model* m, const char* name, float* out_host, int64_t max_elems);
 
