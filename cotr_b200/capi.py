@@ -48,6 +48,8 @@ _PROTOTYPES = {
     "cotr_encode_images": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p]),
     "cotr_encode_context_pairs": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p, ctypes.c_int,
                                                  ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p]),
+    "cotr_decode_ragged": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int,
+                                          ctypes.c_void_p, ctypes.c_void_p]),
     "cotr_forward": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p]),
     "cotr_forward_host": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_void_p]),
     "cotr_preprocess": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_void_p, ctypes.c_int,
@@ -185,6 +187,16 @@ class NativeModel:
         B, Q = queries.shape[0], queries.shape[1]
         pred = torch.empty((B, Q, 2), dtype=torch.float32, device=queries.device)
         check(lib().cotr_decode(self.handle, ctx.handle, _ptr(queries), B, Q, _ptr(pred), self._stream()), "cotr_decode")
+        return pred
+
+    def decode_ragged(self, ctx, queries, offsets):
+        """Pair p's queries are rows offsets[p] .. offsets[p+1]-1 of the packed (R,2) device tensor `queries`, R = offsets[B];
+        offsets: B+1 integers (host) -> packed (R,2) predictions (cotr_decode_ragged)."""
+        off = np.ascontiguousarray(offsets, dtype=np.int64).reshape(-1)
+        R = max(int(off[-1]), 0) if off.size else 0          # the library checks the offsets
+        pred = torch.empty((R, 2), dtype=torch.float32, device=queries.device)
+        check(lib().cotr_decode_ragged(self.handle, ctx.handle, _ptr(queries), ctypes.c_void_p(off.ctypes.data), off.size - 1,
+                                       _ptr(pred), self._stream()), "cotr_decode_ragged")
         return pred
 
     def encode_context_attention(self, img, ctx, layer_mask):

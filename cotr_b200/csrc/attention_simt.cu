@@ -7,7 +7,7 @@ namespace cotr {
 
 namespace {
 
-constexpr int kRowsPerCta = 64;
+constexpr int kRowsPerCta = kAttnSimtTileRows;   // 64
 constexpr int kWarps = 8;
 constexpr int kKStride = kHeadDim + 1;   // padded: lane j reads key (j + 32 i) without bank conflicts
 
@@ -24,9 +24,16 @@ __global__ void __launch_bounds__(kWarps * 32) attention_simt_kernel(const AttnP
     float* Qs = Vs + kTokens * kHeadDim;               // [kWarps][32]
 
     const int head = blockIdx.y;
-    const int pair_local = blockIdx.z;
-    const int row_begin = blockIdx.x * kRowsPerCta;
-    const int row_end = min(row_begin + kRowsPerCta, p.nq);
+    // this CTA's query rows: q / out rows qrow0 .. qrow0 + nrows - 1 (at most kRowsPerCta)
+    int pair_local, qrow0, nrows;
+    if (p.tiles) {
+        const int4 tl = p.tiles[blockIdx.x];
+        pair_local = tl.x; qrow0 = tl.y; nrows = tl.z;
+    } else {
+        pair_local = blockIdx.z;
+        qrow0 = pair_local * p.nq + blockIdx.x * kRowsPerCta;
+        nrows = min(kRowsPerCta, p.nq - blockIdx.x * kRowsPerCta);
+    }
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
 
     const size_t kv_row0 = (size_t)(p.pair0 + pair_local) * kTokens;
@@ -62,8 +69,8 @@ __global__ void __launch_bounds__(kWarps * 32) attention_simt_kernel(const AttnP
     __syncthreads();
 
     float* qs = Qs + warp * kHeadDim;
-    for (int i = row_begin + warp; i < row_end; i += kWarps) {
-        const size_t r = (size_t)pair_local * p.nq + i;
+    for (int i = warp; i < nrows; i += kWarps) {
+        const size_t r = (size_t)qrow0 + i;
         qs[lane] = join_f16(p.q.hi[r * p.ldq + head * kHeadDim + lane], p.q.lo[r * p.ldq + head * kHeadDim + lane]);
         __syncwarp();
         float s[kTokens / 32];
@@ -105,13 +112,13 @@ constexpr size_t kSmemBytes = (size_t)(kTokens * kKStride + kTokens * kHeadDim +
 }  // namespace
 
 int launch_attention_simt(const AttnParams& p, cudaStream_t s) {
-    if (p.nq <= 0 || p.npairs <= 0) return 0;
+    if (p.tiles ? p.n_tiles <= 0 : (p.nq <= 0 || p.npairs <= 0)) return 0;
     static unsigned long long configured = 0;      // bit per device
     if (first_use_on_device(&configured)) {
         COTR_CHECK_CUDA(cudaFuncSetAttribute(attention_simt_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes));
     }
-    COTR_CHECK(p.npairs <= 65535, "attention: too many pairs in one launch (%d)", p.npairs);
-    dim3 grid((p.nq + kRowsPerCta - 1) / kRowsPerCta, kHeads, p.npairs);
+    COTR_CHECK(p.tiles || p.npairs <= 65535, "attention: too many pairs in one launch (%d)", p.npairs);
+    const dim3 grid = p.tiles ? dim3(p.n_tiles, kHeads, 1) : dim3((p.nq + kRowsPerCta - 1) / kRowsPerCta, kHeads, p.npairs);
     COTR_CHECK_CUDA(launch_kernel(attention_simt_kernel, grid, dim3(kWarps * 32), kSmemBytes, s, p));
     return 0;
 }

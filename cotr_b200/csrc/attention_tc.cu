@@ -28,7 +28,7 @@ namespace {
 
 using namespace tc;
 
-constexpr int kTile = 128;
+constexpr int kTile = kAttnTcTileRows;                    // 128
 constexpr int kThreads = 256;                             // two warpgroups
 constexpr int kChunk = 64;                                // keys per softmax chunk
 constexpr int kChunks = kTokens / kChunk;                 // 8
@@ -81,11 +81,19 @@ __global__ void __maxnreg__(168) attention_tc_kernel(const AttnParams p) {
     const int t = threadIdx.x;
     const int warp = t >> 5, lane = t & 31;
     const int head = blockIdx.y;
-    const int pair_local = blockIdx.z / KS;
     const int rank = blockIdx.z % KS;                     // rank in the cluster (1 x 1 x KS)
     const int key0 = rank * kKeys;
     const int chunk0 = rank * kMyChunks;
-    const int row0 = blockIdx.x * kTile;
+    // this CTA's query rows: q / out rows qrow0 .. qrow0 + nrows - 1 (at most kTile of them; the rest of the tile is masked)
+    int pair_local, qrow0, nrows;
+    if (p.tiles) {
+        const int4 tl = p.tiles[blockIdx.x];
+        pair_local = tl.x; qrow0 = tl.y; nrows = tl.z;
+    } else {
+        pair_local = blockIdx.z / KS;
+        qrow0 = pair_local * p.nq + blockIdx.x * kTile;
+        nrows = p.nq - blockIdx.x * kTile;
+    }
 
     if (t == 0) {
         mbar_init(qk_full, kThreads);
@@ -122,9 +130,8 @@ __global__ void __maxnreg__(168) attention_tc_kernel(const AttnParams p) {
     // ---- stage Q (row t % 128, two of the four 16-byte K groups per thread) and K (kKeys / 128 keys per thread) -----
     {
         const int r = t & 127, kg0 = (t >> 7) * 2;
-        const int qr = row0 + r;
-        const bool ok = qr < p.nq;
-        const size_t qoff = ((size_t)pair_local * p.nq + (ok ? qr : 0)) * p.ldq + head * kHeadDim;
+        const bool ok = r < nrows;
+        const size_t qoff = ((size_t)qrow0 + (ok ? r : 0)) * p.ldq + head * kHeadDim;
         const uint32_t bytes = ok ? 16u : 0u;
 #pragma unroll
         for (int j = 0; j < 2; ++j) {
@@ -315,10 +322,10 @@ __global__ void __maxnreg__(168) attention_tc_kernel(const AttnParams p) {
         const float inv_a = 1.f / sum_a, inv_b = 1.f / sum_b;
 #pragma unroll
         for (int h = 0; h < 2; ++h) {                  // row a, row b
-            const int qi = row0 + ra + 8 * h;
-            if (qi >= p.nq) continue;
+            const int qi = ra + 8 * h;
+            if (qi >= nrows) continue;
             const float inv = h ? inv_b : inv_a;
-            const size_t ooff = ((size_t)pair_local * p.nq + qi) * p.ldo + head * kHeadDim + 2 * (lane & 3);
+            const size_t ooff = ((size_t)qrow0 + qi) * p.ldo + head * kHeadDim + 2 * (lane & 3);
 #pragma unroll
             for (int j = 0; j < 4; ++j) {
                 const int i0 = 4 * j + 2 * h;
@@ -348,12 +355,19 @@ int launch_split(const AttnParams& p, dim3 grid, cudaStream_t s) {
 }  // namespace
 
 int launch_attention_tc(const AttnParams& p, cudaStream_t s) {
-    if (p.nq <= 0 || p.npairs <= 0) return 0;
-    if (p.nq < 32) return launch_attention_simt(p, s);   // a 128-row MMA tile would be > 75% padding
-    COTR_CHECK(p.npairs <= 65535, "attention: too many pairs in one launch (%d)", p.npairs);
+    dim3 grid;
+    if (p.tiles) {
+        // ragged decode: the caller has already sent the pairs with < kAttnTcMinRows rows to the SIMT kernel
+        if (p.n_tiles <= 0) return 0;
+        grid = dim3(p.n_tiles, kHeads, 1);
+    } else {
+        if (p.nq <= 0 || p.npairs <= 0) return 0;
+        if (p.nq < kAttnTcMinRows) return launch_attention_simt(p, s);   // a 128-row MMA tile would be > 75% padding
+        COTR_CHECK(p.npairs <= 65535, "attention: too many pairs in one launch (%d)", p.npairs);
+        grid = dim3((p.nq + kTile - 1) / kTile, kHeads, p.npairs);
+    }
     COTR_CHECK((p.ldq & 7) == 0 && (p.ldk & 7) == 0 && (p.ldo & 7) == 0 && (p.vt_pair_stride & 7) == 0,
                "attention_tc: leading dimensions must be multiples of 8 elements");
-    dim3 grid((p.nq + kTile - 1) / kTile, kHeads, p.npairs);
     // Key split over a cluster pair for launches that leave SMs idle (one CTA per SM: shared memory), as long as the
     // doubled grid still fits one wave.  No split by 4: at this shared-memory size an H100 SXM holds only 30 clusters
     // of 4 CTAs at once (cudaOccupancyMaxActiveClusters), so the batch-1 encoder's 32 would take two waves.

@@ -213,9 +213,15 @@ struct GemmParams {
     unsigned char* kv_img;
 };
 
+// Query rows per CTA of the two attention kernels, and the fewest rows of one pair that go to the tensor-core kernel
+// (fewer: a 128-row MMA tile would be more than 75% padding, the SIMT kernel runs them).
+constexpr int kAttnTcTileRows = 128;
+constexpr int kAttnSimtTileRows = 64;
+constexpr int kAttnTcMinRows = 32;
+
 // softmax(q k^T) v per head; q already carries the head_dim^-0.5 scale.
 struct AttnParams {
-    CSplit16 q; int ldq;         // rows: local row r = pair_local * nq + i
+    CSplit16 q; int ldq;         // rows: local row r = pair_local * nq + i (see tiles below)
     CSplit16 k; int ldk;         // rows: (pair0 + pair_local) * 512 + key
     CSplit16 vt;                 // [(pair0 + pair_local) * vt_pair_stride + (head*32 + d) * 512 + key]
     size_t vt_pair_stride;
@@ -227,6 +233,12 @@ struct AttnParams {
     int nq;                      // query rows per pair in this launch
     int npairs;
     int pair0;
+    // Ragged decode (cotr_decode_ragged): when non-null, CTA blockIdx.x owns the rows of tile tiles[blockIdx.x] =
+    // (pair_local, first q / out row, row count) - at most one CTA tile of rows of one pair - and nq / npairs are unused:
+    // the grid is (n_tiles, heads, key split).  Written before the launch by a copy, never by a kernel, so the kernels
+    // may read it before the dependency wait.  null: row r = pair_local * nq + i as above.
+    const int4* tiles;
+    int n_tiles;
 };
 
 // Head-averaged attention weights (attention_weights.cu): out[pair_local][i][key] = (1/8) sum_h softmax(q_h k_h^T)[i][key],

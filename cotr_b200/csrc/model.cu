@@ -146,6 +146,11 @@ struct cotr_model {
     int* pair_stage = nullptr;
     int pair_cap = 0;
     cudaEvent_t pair_copied = nullptr;
+    // cotr_decode_ragged: the attention tile tables of all chunks of a call (AttnParams::tiles), staged the same way
+    int4* tile_tab = nullptr;
+    int4* tile_stage = nullptr;
+    size_t tile_cap = 0;
+    cudaEvent_t tile_copied = nullptr;
     cotr::Preprocessor* pre = nullptr;         // device-side crop / resize / normalise (cotr_preprocess)
     cotr::FlowMerger* merger = nullptr;        // device-side tail of the dense first guess (cotr_flow_tile_merge)
     bool prof_on = false;
@@ -462,6 +467,30 @@ int run_attention(const Run& r, const AttnParams& p) {
     LaunchScope scope(r, r.m->gemm_path == 0 ? K_ATTN_TC : K_ATTN_SIMT, p.nq * p.npairs, kTokens, kDModel);
     if (r.m->gemm_path != 0) return launch_attention_simt(p, r.s);
     return launch_attention_tc(p, r.s);
+}
+
+// The attention tiles of one ragged decode chunk (cotr_decode_ragged): a device table of n_tc tensor-core tiles
+// (kAttnTcTileRows rows of a pair with >= kAttnTcMinRows rows in the chunk) followed by n_simt SIMT tiles
+// (kAttnSimtTileRows rows: the other pairs, or every pair on the fp32 SIMT path), see AttnParams::tiles.
+struct ChunkTiles {
+    const int4* tab = nullptr;
+    int n_tc = 0, n_simt = 0;
+    int rows_tc = 0, rows_simt = 0;
+};
+
+// One launch per kind of tile present; the two launches write disjoint rows of the output.
+int run_attention_tiles(const Run& r, AttnParams a, const ChunkTiles& t) {
+    if (t.n_tc > 0) {
+        a.tiles = t.tab; a.n_tiles = t.n_tc;
+        LaunchScope scope(r, K_ATTN_TC, t.rows_tc, kTokens, kDModel);
+        if (launch_attention_tc(a, r.s)) return 1;
+    }
+    if (t.n_simt > 0) {
+        a.tiles = t.tab + t.n_tc; a.n_tiles = t.n_simt;
+        LaunchScope scope(r, K_ATTN_SIMT, t.rows_simt, kTokens, kDModel);
+        if (launch_attention_simt(a, r.s)) return 1;
+    }
+    return 0;
 }
 
 // Where the head-averaged attention maps of the selected layers go (cotr_encode_context_attention /
@@ -862,13 +891,15 @@ int encode_pairs_impl(cotr_model* m, const void* feat_dev, int n_images, const i
     return encode_tail(m, CSplit16{hi, hi + (size_t)n_images * kFeatElems}, m->pair_tab, B, ctx, s, maps);
 }
 
+// R query rows (queries / pred: (R,2)).  tiles == nullptr: pair pair0 + p owns rows p * nq .. p * nq + nq - 1, p < npairs;
+// otherwise the attention follows the chunk's tile table (a ragged chunk, no maps) and pair0 / npairs / nq are unused.
 // maps.base: this chunk's first row (pair pair0, its first query) in the caller's (n_sel, B, Q, 512) buffer
-int decode_chunk(cotr_model* m, const cotr_context* ctx, const float* queries, float* pred, int pair0, int npairs,
-                 int nq, cudaStream_t s, const AttnMaps& maps) {
+int decode_chunk(cotr_model* m, const cotr_context* ctx, const float* queries, float* pred, int R, const ChunkTiles* tiles,
+                 int pair0, int npairs, int nq, cudaStream_t s, const AttnMaps& maps) {
     Workspace& w = m->ws;
     Run r{m, s};
-    const int R = npairs * nq;
     const CSplit16 none{nullptr, nullptr};
+    auto attend = [&](const AttnParams& a) { return tiles ? run_attention_tiles(r, a, *tiles) : run_attention(r, a); };
     // cotr_model.py:34-35 query_proj (lin_sine, depth 64)
     {
         LaunchScope scope(r, K_QENC, R, kDModel, 0);
@@ -898,7 +929,7 @@ int decode_chunk(cotr_model* m, const cotr_context* ctx, const float* queries, f
             if (ctx->holds_img) { a.kv_img = ctx->img + (size_t)l * kHeads * kAttnHeadImgBytes; a.img_pair_stride = (size_t)kDecLayers * kHeads * kAttnHeadImgBytes; }
             a.out = w.dao; a.ldo = kDModel;
             a.nq = nq; a.npairs = npairs; a.pair0 = pair0;
-            if (run_attention(r, a)) return 1;
+            if (attend(a)) return 1;
             if (run_attention_weights(r, a, maps, l)) return 1;
             // transformer.py:196-197: t = t + out_proj(attn)   (norm2 deferred; t = norm3_{l-1}(t2), deferred, or 0)
             if (run_linear_dln(r, d.o, R, cs(w.dao), kDModel, w.t, kDModel, false, nullptr, w.dec_st_a, ln_in ? cs(w.t2) : none, kDModel,
@@ -931,7 +962,7 @@ int decode_chunk(cotr_model* m, const cotr_context* ctx, const float* queries, f
             if (ctx->holds_img) { a.kv_img = ctx->img + (size_t)l * kHeads * kAttnHeadImgBytes; a.img_pair_stride = (size_t)kDecLayers * kHeads * kAttnHeadImgBytes; }
             a.out = w.dao; a.ldo = kDModel;
             a.nq = nq; a.npairs = npairs; a.pair0 = pair0;
-            if (run_attention(r, a)) return 1;
+            if (attend(a)) return 1;
             if (run_attention_weights(r, a, maps, l)) return 1;
             // transformer.py:196-197: t = norm2(t + out_proj(attn))
             if (run_linear(r, d.o, R, cs(w.dao), kDModel, w.t, kDModel, false, l > 0 ? cs(w.t) : none, kDModel, d.ln2_g, d.ln2_b, w.dln_tmp)) return 1;
@@ -980,7 +1011,7 @@ int decode_impl(cotr_model* m, const cotr_context* ctx, const float* queries, in
         const int pairs_per = kDecodeChunkRows / Q;
         for (int b0 = 0; b0 < B; b0 += pairs_per) {
             const int nb = (B - b0 < pairs_per) ? B - b0 : pairs_per;
-            if (decode_chunk(m, ctx, queries + (size_t)b0 * Q * 2, pred + (size_t)b0 * Q * 2, b0, nb, Q, s,
+            if (decode_chunk(m, ctx, queries + (size_t)b0 * Q * 2, pred + (size_t)b0 * Q * 2, nb * Q, nullptr, b0, nb, Q, s,
                              maps.at((size_t)b0 * Q * kTokens))) return 1;
         }
     } else {
@@ -988,10 +1019,98 @@ int decode_impl(cotr_model* m, const cotr_context* ctx, const float* queries, in
             for (int q0 = 0; q0 < Q; q0 += kDecodeChunkRows) {
                 const int nq = (Q - q0 < kDecodeChunkRows) ? Q - q0 : kDecodeChunkRows;
                 const size_t off = ((size_t)b * Q + q0) * 2;
-                if (decode_chunk(m, ctx, queries + off, pred + off, b, 1, nq, s, maps.at(((size_t)b * Q + q0) * kTokens))) return 1;
+                if (decode_chunk(m, ctx, queries + off, pred + off, nq, nullptr, b, 1, nq, s, maps.at(((size_t)b * Q + q0) * kTokens))) return 1;
             }
     }
     m->last_rows = (total <= kDecodeChunkRows) ? (int)total : 0;
+    return 0;
+}
+
+// Ragged decode (cotr_decode_ragged): pair p owns the packed rows offsets[p] .. offsets[p+1] - 1.  Whole pairs are packed in
+// order into chunks of at most kDecodeChunkRows rows; a pair with more rows than that gets chunks of its own, one per
+// slice, as in decode_impl.  A chunk is a contiguous row range, so its queries and predictions are pointer offsets, and
+// with the same count Q for every pair the chunks, and so the launches, are exactly those of decode_impl.  Every chunk's
+// attention tile table is built on the host and reaches the device with one copy per call.  Arguments are checked by
+// the caller.
+int decode_ragged_impl(cotr_model* m, const cotr_context* ctx, const float* queries, const int64_t* offsets, int B,
+                       float* pred, cudaStream_t s) {
+    struct Chunk {
+        int64_t row0 = 0;      // first packed row
+        int rows = 0;
+        size_t tab0 = 0;       // first entry of the chunk's tiles in the call's table
+        ChunkTiles t;
+    };
+    struct Segment { int pair, row0, rows; };     // rows of one pair in a chunk, row0 relative to the chunk
+    std::vector<Chunk> chunks;
+    std::vector<int4> tab;
+    std::vector<Segment> segs;
+    const bool tc = m->gemm_path == 0;
+    Chunk cur;
+    auto close = [&]() {
+        if (cur.rows == 0) return;
+        cur.tab0 = tab.size();
+        // tensor-core tiles first, then the SIMT tiles (see ChunkTiles)
+        for (int pass = 0; pass < 2; ++pass) {
+            const size_t first = tab.size();
+            for (const Segment& g : segs) {
+                const bool to_tc = tc && g.rows >= kAttnTcMinRows;
+                if (to_tc != (pass == 0)) continue;
+                const int step = to_tc ? kAttnTcTileRows : kAttnSimtTileRows;
+                for (int i = 0; i < g.rows; i += step) tab.push_back(make_int4(g.pair, g.row0 + i, std::min(step, g.rows - i), 0));
+                (to_tc ? cur.t.rows_tc : cur.t.rows_simt) += g.rows;
+            }
+            (pass == 0 ? cur.t.n_tc : cur.t.n_simt) = (int)(tab.size() - first);
+        }
+        chunks.push_back(cur);
+        const int64_t next = cur.row0 + cur.rows;
+        cur = Chunk();
+        cur.row0 = next;
+        segs.clear();
+    };
+    for (int p = 0; p < B; ++p) {
+        const int64_t n = offsets[p + 1] - offsets[p];
+        if (n == 0) continue;
+        if (n > kDecodeChunkRows) {
+            close();
+            for (int64_t q0 = 0; q0 < n; q0 += kDecodeChunkRows) {
+                const int rows = (int)std::min<int64_t>(kDecodeChunkRows, n - q0);
+                segs.push_back({p, 0, rows});
+                cur.rows = rows;
+                close();
+            }
+            continue;
+        }
+        if (cur.rows + n > kDecodeChunkRows) close();
+        segs.push_back({p, cur.rows, (int)n});
+        cur.rows += (int)n;
+    }
+    close();
+
+    int cap = 0;
+    for (const Chunk& c : chunks) cap = std::max(cap, c.rows);
+    if (ensure_decode_ws(m, cap)) return 1;
+    if (tab.size() > m->tile_cap) {
+        COTR_CHECK_CUDA(cudaDeviceSynchronize());
+        m->tile_cap = 0;      // as in ensure_decode_ws: no stale capacity after a failed allocation
+        if (m->tile_tab) { cudaFree(m->tile_tab); m->tile_tab = nullptr; }
+        if (m->tile_stage) { cudaFreeHost(m->tile_stage); m->tile_stage = nullptr; }
+        COTR_CHECK_CUDA(cudaMalloc((void**)&m->tile_tab, tab.size() * sizeof(int4)));
+        COTR_CHECK_CUDA(cudaMallocHost((void**)&m->tile_stage, tab.size() * sizeof(int4)));
+        m->tile_cap = tab.size();
+    }
+    if (!m->tile_copied) COTR_CHECK_CUDA(cudaEventCreateWithFlags(&m->tile_copied, cudaEventDisableTiming));
+    // as in encode_pairs_impl: the previous call's copy out of the staging buffer has long completed unless the host
+    // runs a whole call ahead of the device
+    COTR_CHECK_CUDA(cudaEventSynchronize(m->tile_copied));
+    memcpy(m->tile_stage, tab.data(), tab.size() * sizeof(int4));
+    COTR_CHECK_CUDA(cudaMemcpyAsync(m->tile_tab, m->tile_stage, tab.size() * sizeof(int4), cudaMemcpyHostToDevice, s));
+    COTR_CHECK_CUDA(cudaEventRecord(m->tile_copied, s));
+    for (Chunk& c : chunks) {
+        c.t.tab = m->tile_tab + c.tab0;
+        const size_t off = (size_t)c.row0 * 2;
+        if (decode_chunk(m, ctx, queries + off, pred + off, c.rows, &c.t, 0, 0, 0, s, AttnMaps())) return 1;
+    }
+    m->last_rows = chunks.size() == 1 ? chunks[0].rows : 0;
     return 0;
 }
 
@@ -1220,6 +1339,9 @@ void cotr_destroy(cotr_model* m) {
     if (m->pair_tab) cudaFree(m->pair_tab);
     if (m->pair_stage) cudaFreeHost(m->pair_stage);
     if (m->pair_copied) cudaEventDestroy(m->pair_copied);
+    if (m->tile_tab) cudaFree(m->tile_tab);
+    if (m->tile_stage) cudaFreeHost(m->tile_stage);
+    if (m->tile_copied) cudaEventDestroy(m->tile_copied);
     float** fbufs[] = {&w.ln_tmp, &w.dln_tmp, &w.img_stage, &w.q_stage, &w.pred_stage,
                        reinterpret_cast<float**>(&w.enc_st_a), reinterpret_cast<float**>(&w.enc_st_b),
                        reinterpret_cast<float**>(&w.dec_st_a), reinterpret_cast<float**>(&w.dec_st_b)};
@@ -1272,6 +1394,29 @@ int cotr_decode(cotr_model* m, const cotr_context* ctx, const float* queries_dev
     CallOrder order(m, (cudaStream_t)cuda_stream);
     m->launches = 0;
     return decode_impl(m, ctx, queries_dev, B, Q, pred_dev, (cudaStream_t)cuda_stream);
+}
+
+int cotr_decode_ragged(cotr_model* m, const cotr_context* ctx, const float* queries_dev, const int64_t* offsets_host, int B,
+                       float* pred_dev, void* cuda_stream) {
+    const char* fn = "cotr_decode_ragged";
+    COTR_CHECK(m != nullptr, "%s: null model", fn);
+    m->launches = 0;
+    COTR_CHECK(ctx && ctx->model == m, "%s: context does not belong to this model", fn);
+    COTR_CHECK(B >= 1 && B == ctx->pairs, "%s: B = %d but the context holds %d pairs", fn, B, ctx->pairs);
+    COTR_CHECK(ctx->holds_img == (m->gemm_path == 0), "%s: the context was encoded under the other matrix-multiply path "
+               "(cotr_set_gemm_path): re-encode it", fn);
+    COTR_CHECK(offsets_host != nullptr, "%s: null offsets_host", fn);
+    COTR_CHECK(offsets_host[0] == 0, "%s: offsets_host[0] = %lld, must be 0", fn, (long long)offsets_host[0]);
+    for (int p = 0; p < B; ++p)
+        COTR_CHECK(offsets_host[p + 1] >= offsets_host[p], "%s: offsets_host decreases at pair %d (%lld -> %lld)", fn, p,
+                   (long long)offsets_host[p], (long long)offsets_host[p + 1]);
+    const int64_t R = offsets_host[B];
+    COTR_CHECK(R <= INT32_MAX, "%s: %lld query rows in one call (at most %d)", fn, (long long)R, INT32_MAX);
+    if (R == 0) return 0;
+    COTR_CHECK(queries_dev && pred_dev, "%s: null queries_dev or pred_dev for %lld rows", fn, (long long)R);
+    COTR_CHECK_CUDA(cudaSetDevice(m->device));
+    CallOrder order(m, (cudaStream_t)cuda_stream);
+    return decode_ragged_impl(m, ctx, queries_dev, offsets_host, B, pred_dev, (cudaStream_t)cuda_stream);
 }
 
 namespace {

@@ -24,7 +24,8 @@ kwargs = {} for with_kwargs hooks, and output = (None, weights): weights is (B, 
 never materialised.  A hook's return value is ignored.  `encode_context` fires the encoder hooks and `decode` the
 decoder hooks, so a caller that encodes once and decodes twice (cotr_corr_base's cycle pass) sees the encoder hooks
 fire once where the reference fires them twice.  Without hooks nothing of this runs.  Forward pre-hooks and the
-sharded model are not covered.
+sharded model are not covered, and a ragged `decode` (a list of per-pair query sets) refuses decoder hooks: it
+produces no attention maps.
 """
 import itertools
 import math
@@ -404,8 +405,28 @@ class COTR(nn.Module):
 
     @torch.no_grad()
     def decode(self, ctx, queries):
+        """queries: a (B,Q,2) tensor, or a list / tuple of B tensors (Q_p,2) with a count Q_p >= 0 per pair (ragged
+        decode, cotr_decode_ragged); then pred_corrs is a list of B (Q_p,2) views of one packed output tensor."""
+        if isinstance(queries, (list, tuple)):
+            return {'pred_corrs': self._decode_ragged(ctx, queries)}
         q = self._queries(queries, ctx.batch)
         return {'pred_corrs': self._decode(ctx.native, q)}
+
+    def _decode_ragged(self, ctx, queries):
+        assert len(queries) == ctx.batch, f"ragged queries: {len(queries)} query sets for a context of {ctx.batch} pairs"
+        for i, q in enumerate(queries):
+            assert isinstance(q, torch.Tensor) and q.ndim == 2 and q.shape[1] == 2, \
+                f"ragged queries: set {i} must be a (Q,2) tensor, got {tuple(getattr(q, 'shape', ()))}"
+        _, dec = self._attention_modules()
+        if self._hooked(dec):
+            raise RuntimeError("decode: attention maps are not produced for ragged decodes (list of query sets); remove the "
+                               "decoder attention hooks or decode a (B,Q,2) tensor")
+        dev = next(self.parameters()).device
+        counts = [int(q.shape[0]) for q in queries]
+        packed = torch.cat([q.to(device=dev, dtype=torch.float32) for q in queries]).contiguous()
+        offsets = np.concatenate([[0], np.cumsum(counts)]).astype(np.int64)
+        pred = self.native().decode_ragged(ctx.native, packed, offsets)
+        return list(pred.split(counts))
 
 
 def build(args):

@@ -117,6 +117,17 @@ int cotr_encode_images(cotr_model* m, const float* img_dev, int N, void* feat_de
 int cotr_encode_context_pairs(cotr_model* m, const void* feat_dev, int n_images, const int32_t* pairs_host, int B,
                               cotr_context* ctx, int layer_mask, float* attn_dev, void* cuda_stream);
 
+/* Ragged decode: a different number of queries for each pair of a context in one call (the keypoints of each image of a
+ * set, the surviving predictions of a cycle pass).  queries_dev: (R,2), pred_dev: (R,2), R = offsets_host[B]; pair p's
+ * queries are rows offsets_host[p] .. offsets_host[p+1]-1.  B must equal the context's pair count; offsets_host (B+1
+ * int64, HOST) starts at 0 and never decreases (empty pairs are allowed).  A pair's predictions do not depend on the
+ * other pairs' queries: with the same count Q for every pair the call launches exactly the kernels of cotr_decode and
+ * its predictions are bitwise cotr_decode's.  All arguments are checked on the host before anything is enqueued;
+ * R == 0 returns 0 without a launch.  The attention tile table of the call goes to the device through a pinned staging
+ * buffer, with the same wait as cotr_encode_context_pairs.  No attention maps.  Eager (no CUDA-graph capture). */
+int cotr_decode_ragged(cotr_model* m, const cotr_context* ctx, const float* queries_dev, const int64_t* offsets_host,
+                       int B, float* pred_dev, void* cuda_stream);
+
 /* cotr_encode_context + cotr_decode on an internal context. */
 int cotr_forward(cotr_model* m, const float* img_dev, const float* queries_dev, int B, int Q,
                  float* pred_dev, void* cuda_stream);
