@@ -25,6 +25,16 @@ class TestGemmDesc(ctypes.Structure):
         "relu", "add_period", "ld_add", "ldr", "ldc", "a_ln", "res_ln", "emit_part", "reserved")] + [("a_elems", ctypes.c_int64)]
 
 
+class TestAttentionDesc(ctypes.Structure):
+    _fields_ = [(n, ctypes.c_int32) for n in (
+        "path", "nq", "npairs", "operands", "slots", "slot", "ctx_pairs", "pair0", "q_rows", "ldq", "q_col0", "n_tiles",
+        "key_split", "reserved")]
+
+
+class TestMlpDesc(ctypes.Structure):
+    _fields_ = [(n, ctypes.c_int32) for n in ("M", "rows", "split", "in_place")]
+
+
 class LaunchRecord(ctypes.Structure):
     _fields_ = [("kernel", ctypes.c_int32), ("M", ctypes.c_int32), ("N", ctypes.c_int32), ("K", ctypes.c_int32),
                 ("ms", ctypes.c_float)]
@@ -76,7 +86,9 @@ _PROTOTYPES = {
     "cotr_debug_read": (ctypes.c_int64, [ctypes.c_void_p, ctypes.c_char_p, ctypes.c_void_p, ctypes.c_int64]),
     "cotr_set_gemm_path": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_int]),
     "cotr_test_gemm": (ctypes.c_int, [ctypes.POINTER(TestGemmDesc)] + [ctypes.c_void_p] * 9),
-    "cotr_test_attention": (ctypes.c_int, [ctypes.c_int] + [ctypes.c_void_p] * 4 + [ctypes.c_int, ctypes.c_int]),
+    "cotr_test_attention": (ctypes.c_int, [ctypes.POINTER(TestAttentionDesc)] + [ctypes.c_void_p] * 5),
+    "cotr_test_mlp": (ctypes.c_int, [ctypes.POINTER(TestMlpDesc)] + [ctypes.c_void_p] * 10),
+    "cotr_test_rowwise": (ctypes.c_int, [ctypes.c_int, ctypes.c_int] + [ctypes.c_void_p] * 6),
     "cotr_test_attention_weights": (ctypes.c_int, [ctypes.c_int] + [ctypes.c_void_p] * 3 + [ctypes.c_int, ctypes.c_int]),
     "cotr_debug_set_variant": (None, [ctypes.c_int]),
     "cotr_last_error": (ctypes.c_char_p, []),
@@ -455,7 +467,65 @@ def test_attention_weights(path, q, k, nq, npairs):
     return out
 
 
-def test_attention(path, q, k, v, nq, npairs):
-    out = torch.zeros_like(q)
-    check(lib().cotr_test_attention(path, _ptr(q), _ptr(k), _ptr(v), _ptr(out), nq, npairs), "cotr_test_attention")
+ATTENTION_OPERANDS = {"rowmajor": 0, "images": 1}
+
+
+def test_attention(path, q, k, v, nq, npairs, *, operands="rowmajor", pair0=0, slot=0, q_col0=0, tiles=None, key_split=0,
+                   out=None):
+    """Kernel-level hook: softmax(q k^T) v per head, launched as the model launches it (cotr_test_attention).
+
+    q: (rows, ldq) CUDA fp32, the launch reads columns q_col0 .. q_col0+255.  k, v: (ctx_pairs*512, slots*256) CUDA fp32,
+    the keys / values of `slots` layers side by side per pair as in a context; the launch reads slot `slot` of pairs
+    pair0 .. .  operands: "rowmajor" (fp32 SIMT schedule) or "images" (tensor-core schedule).  tiles: optional (n,3)
+    table of (pair, first row, row count) - then nq / npairs are unused.  key_split (path 0): 0 = launch rule, 1 or 2.
+    out: (rows,256) CUDA fp32, rows the launch does not own are returned unchanged (default zeros)."""
+    d = TestAttentionDesc()
+    d.path, d.nq, d.npairs = path, nq, npairs
+    d.operands = ATTENTION_OPERANDS[operands]
+    d.slots, d.slot = k.shape[1] // 256, slot
+    d.ctx_pairs, d.pair0 = k.shape[0] // 512, pair0
+    d.q_rows, d.ldq, d.q_col0 = q.shape[0], q.shape[1], q_col0
+    d.key_split = key_split
+    assert k.shape == v.shape and k.shape[0] % 512 == 0 and k.shape[1] % 256 == 0
+    assert all(t.is_cuda and t.dtype == torch.float32 and t.is_contiguous() for t in (q, k, v))
+    tab = None
+    if tiles is not None:
+        tab = np.ascontiguousarray(tiles, dtype=np.int32).reshape(-1, 3)
+        d.n_tiles = tab.shape[0]
+    if out is None:
+        out = torch.zeros((q.shape[0], 256), dtype=torch.float32, device=q.device)
+    assert out.is_contiguous() and out.shape == (q.shape[0], 256)
+    check(lib().cotr_test_attention(ctypes.byref(d), _ptr(q), _ptr(k), _ptr(v), _ptr(out),
+                                    ctypes.c_void_p(tab.ctypes.data) if tab is not None else None), "cotr_test_attention")
+    return out
+
+
+def test_mlp(x, M, w1, b1, w2, b2, g, be, g2=None, be2=None, *, split=0, in_place=False, out=None):
+    """Kernel-level hook: the fused feed-forward block (cotr_test_mlp) on rows < M of x (rows, 256):
+    LN(x + relu(x w1^T + b1) w2^T + b2), then LN(., g2, be2) when given.  w1 (1024,256) / w2 (256,1024) host arrays, the
+    other operands CUDA fp32.  split: 0 = launch rule, 4 or 8 CTAs per row tile.  in_place: the launch writes into x.
+    out: (rows,256), rows >= M are returned unchanged (in place: x's rows) (default zeros)."""
+    d = TestMlpDesc()
+    d.M, d.rows, d.split, d.in_place = M, x.shape[0], split, int(in_place)
+    if out is None:
+        out = torch.zeros_like(x)
+    assert x.is_contiguous() and out.is_contiguous() and x.shape == out.shape and x.shape[1] == 256
+    w1 = np.ascontiguousarray(w1, np.float32)
+    w2 = np.ascontiguousarray(w2, np.float32)
+    assert w1.shape == (1024, 256) and w2.shape == (256, 1024)
+    p = lambda t: _ptr(t) if t is not None else None
+    check(lib().cotr_test_mlp(ctypes.byref(d), _ptr(x), ctypes.c_void_p(w1.ctypes.data), _ptr(b1), ctypes.c_void_p(w2.ctypes.data),
+                              _ptr(b2), _ptr(g), _ptr(be), p(g2), p(be2), _ptr(out)), "cotr_test_mlp")
+    return out
+
+
+ROWWISE_OPS = {"layernorm": 0, "layernorm_f32": 1, "layernorm_twice": 2, "query_encode": 3}
+
+
+def test_rowwise(op, x, g1=None, b1=None, g2=None, b2=None):
+    """Kernel-level hook: a row kernel (cotr_test_rowwise) on x (rows,256), or on (rows,2) points for query_encode
+    -> (rows,256)."""
+    out = torch.zeros((x.shape[0], 256), dtype=torch.float32, device=x.device)
+    p = lambda t: _ptr(t) if t is not None else None
+    check(lib().cotr_test_rowwise(ROWWISE_OPS[op], x.shape[0], _ptr(x), p(g1), p(b1), p(g2), p(b2), _ptr(out)), "cotr_test_rowwise")
     return out

@@ -354,26 +354,33 @@ int launch_split(const AttnParams& p, dim3 grid, cudaStream_t s) {
 
 }  // namespace
 
+// CTAs of one key slice: (tiles, heads, pairs); an empty launch has none
+static dim3 tc_grid(const AttnParams& p) {
+    if (p.tiles) return dim3(p.n_tiles > 0 ? p.n_tiles : 0, kHeads, 1);
+    if (p.nq <= 0 || p.npairs <= 0) return dim3(0, kHeads, 1);
+    return dim3((p.nq + kTile - 1) / kTile, kHeads, p.npairs);
+}
+
 int launch_attention_tc(const AttnParams& p, cudaStream_t s) {
-    dim3 grid;
-    if (p.tiles) {
-        // ragged decode: the caller has already sent the pairs with < kAttnTcMinRows rows to the SIMT kernel
-        if (p.n_tiles <= 0) return 0;
-        grid = dim3(p.n_tiles, kHeads, 1);
-    } else {
-        if (p.nq <= 0 || p.npairs <= 0) return 0;
-        if (p.nq < kAttnTcMinRows) return launch_attention_simt(p, s);   // a 128-row MMA tile would be > 75% padding
-        COTR_CHECK(p.npairs <= 65535, "attention: too many pairs in one launch (%d)", p.npairs);
-        grid = dim3((p.nq + kTile - 1) / kTile, kHeads, p.npairs);
-    }
-    COTR_CHECK((p.ldq & 7) == 0 && (p.ldk & 7) == 0 && (p.ldo & 7) == 0 && (p.vt_pair_stride & 7) == 0,
-               "attention_tc: leading dimensions must be multiples of 8 elements");
+    // ragged decode (p.tiles): the caller has already sent the pairs with < kAttnTcMinRows rows to the SIMT kernel
+    if (!p.tiles && p.nq > 0 && p.npairs > 0 && p.nq < kAttnTcMinRows)
+        return launch_attention_simt(p, s);           // a 128-row MMA tile would be > 75% padding
     // Key split over a cluster pair for launches that leave SMs idle (one CTA per SM: shared memory), as long as the
     // doubled grid still fits one wave.  No split by 4: at this shared-memory size an H100 SXM holds only 30 clusters
     // of 4 CTAs at once (cudaOccupancyMaxActiveClusters), so the batch-1 encoder's 32 would take two waves.
+    const dim3 grid = tc_grid(p);
     const long long ctas = (long long)grid.x * grid.y * grid.z;
-    if (ctas * 2 <= kNumSms) return launch_split<2>(p, grid, s);
-    return launch_split<1>(p, grid, s);
+    return launch_attention_tc_split(p, ctas * 2 <= kNumSms ? 2 : 1, s);
+}
+
+int launch_attention_tc_split(const AttnParams& p, int ks, cudaStream_t s) {
+    const dim3 grid = tc_grid(p);
+    if (grid.x == 0) return 0;
+    COTR_CHECK(ks == 1 || ks == 2, "attention_tc: key split %d (1 or 2)", ks);
+    COTR_CHECK(p.tiles || p.npairs <= 65535, "attention: too many pairs in one launch (%d)", p.npairs);
+    COTR_CHECK((p.ldq & 7) == 0 && (p.ldk & 7) == 0 && (p.ldo & 7) == 0 && (p.vt_pair_stride & 7) == 0,
+               "attention_tc: leading dimensions must be multiples of 8 elements");
+    return ks == 2 ? launch_split<2>(p, grid, s) : launch_split<1>(p, grid, s);
 }
 
 }  // namespace cotr

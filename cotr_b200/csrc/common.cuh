@@ -279,6 +279,11 @@ int launch_layernorm_f32(const float* x, const float* gamma, const float* beta, 
 int launch_gemm_tc(const GemmParams& p, cudaStream_t s);
 int launch_attention_simt(const AttnParams& p, cudaStream_t s);
 int launch_attention_tc(const AttnParams& p, cudaStream_t s);
+// launch_mlp_tc / launch_attention_tc with the hidden split (S = 4 or 8 CTAs per row tile) / key split (ks = 1 or 2)
+// given instead of chosen; the tensor-core attention then also runs launches of fewer than kAttnTcMinRows rows per
+// pair.  Test hooks.
+int launch_mlp_tc_split(const MlpParams& p, int S, cudaStream_t s);
+int launch_attention_tc_split(const AttnParams& p, int ks, cudaStream_t s);
 int launch_attention_weights_tc(const AttnWeightsParams& p, cudaStream_t s);
 int launch_attention_weights_simt(const AttnWeightsParams& p, cudaStream_t s);
 int launch_maxpool_3x3s2_nhwc(CSplit16 in, Split16 out, int N, int H, int W, int C, cudaStream_t s);

@@ -376,8 +376,12 @@ int launch_mlp_tc(const MlpParams& p, cudaStream_t s) {
     const int tiles = (p.M + BM - 1) / BM;
     int n8 = 0;
     if (max_clusters_of_8(&n8)) return 1;
-    if (tiles <= n8) return launch_split<8>(p, s);
-    return launch_split<4>(p, s);
+    return launch_mlp_tc_split(p, tiles <= n8 ? 8 : 4, s);
+}
+
+int launch_mlp_tc_split(const MlpParams& p, int S, cudaStream_t s) {
+    COTR_CHECK(S == 4 || S == 8, "mlp_tc: hidden split %d (4 or 8)", S);
+    return S == 8 ? launch_split<8>(p, s) : launch_split<4>(p, s);
 }
 
 }  // namespace cotr

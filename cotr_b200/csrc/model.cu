@@ -1902,41 +1902,188 @@ int cotr_test_gemm(const cotr_test_gemm_desc* d, const float* A_dev, const float
     return 0;
 }
 
-// q (npairs*nq,256), k / v (npairs*512,256) fp32 row-major; v is transposed into the [pair][256][512] layout first.
-int cotr_test_attention(int path, const float* q_dev, const float* k_dev, const float* v_dev, float* out_dev,
-                        int nq, int npairs) {
-    COTR_CHECK(q_dev && k_dev && v_dev && out_dev, "cotr_test_attention: null argument");
-    TmpSplit q16, k16, vt16, o16;
-    const size_t qn = (size_t)npairs * nq * kDModel, kn = (size_t)npairs * kTokens * kDModel;
-    if (q16.from_f32(q_dev, qn) || k16.from_f32(k_dev, kn) || vt16.empty(kn) || o16.empty(qn)) return 1;
-    {   // transpose V with an identity "GEMM": vt = (V * I^T) stored through the transposed-block epilogue
-        std::vector<float> eye((size_t)kDModel * kDModel, 0.f);
-        for (int i = 0; i < kDModel; ++i) eye[(size_t)i * kDModel + i] = 1.f;
-        float* ed = nullptr;
-        COTR_CHECK_CUDA(cudaMalloc((void**)&ed, eye.size() * sizeof(float)));
-        COTR_CHECK_CUDA(cudaMemcpy(ed, eye.data(), eye.size() * sizeof(float), cudaMemcpyHostToDevice));
-        TmpSplit v16;
-        if (v16.from_f32(v_dev, kn)) { cudaFree(ed); return 1; }
+namespace {
+// Device allocations of one test hook call, freed on every return (cudaFree waits for the work queued on them).
+struct DevAllocs {
+    std::vector<void*> ptrs;
+    ~DevAllocs() { for (void* p : ptrs) cudaFree(p); }
+    int alloc(void** out, size_t bytes) {
+        COTR_CHECK_CUDA(cudaMalloc(out, bytes));
+        ptrs.push_back(*out);
+        return 0;
+    }
+    int upload(void** out, const void* host, size_t bytes) {
+        if (alloc(out, bytes)) return 1;
+        COTR_CHECK_CUDA(cudaMemcpy(*out, host, bytes, cudaMemcpyHostToDevice));
+        return 0;
+    }
+};
+
+// tensor-core image of a host [N,K] weight, as the model uploads it; returns acc_scale in *scale
+int upload_tc_weight(DevAllocs& mem, const float* w_host, int N, int K, void** wtc, float* scale) {
+    std::vector<uint8_t> img(tc_weight_bytes(N, K));
+    *scale = tc_pack_weight(w_host, N, K, img.data());
+    return mem.upload(wtc, img.data(), img.size());
+}
+
+std::vector<float> identity(int n) {
+    std::vector<float> eye((size_t)n * n, 0.f);
+    for (int i = 0; i < n; ++i) eye[(size_t)i * n + i] = 1.f;
+    return eye;
+}
+}  // namespace
+
+// The attention launch as the model makes it (see cotr_test_attention_desc).  K / V reach the kernel in the layout of
+// the chosen schedule, produced by the same epilogue stores as in the model: V transposed by the fp32 SIMT identity
+// GEMM (operands 0), or K and V of the slot as the operand images of one tensor-core identity GEMM over [K | V]
+// (operands 1), the other slots' images left 0xFF (fp16 NaN).  `out` is converted in before the launch, so every row
+// the launch does not own comes back as it was passed.
+int cotr_test_attention(const cotr_test_attention_desc* d, const float* q_dev, const float* k_dev, const float* v_dev,
+                        float* out_dev, const int32_t* tiles_host) {
+    COTR_CHECK(d && q_dev && k_dev && v_dev && out_dev, "cotr_test_attention: null argument");
+    COTR_CHECK(d->path == 0 || d->path == 1, "cotr_test_attention: path %d (0 tensor cores, 1 fp32 SIMT)", d->path);
+    COTR_CHECK(d->operands == 0 || d->operands == 1, "cotr_test_attention: operands %d (0 row-major, 1 images)", d->operands);
+    COTR_CHECK(d->slots >= 1 && d->slot >= 0 && d->slot < d->slots, "cotr_test_attention: slot %d of %d", d->slot, d->slots);
+    COTR_CHECK(d->ctx_pairs >= 1 && d->pair0 >= 0, "cotr_test_attention: pair0 %d of %d pairs", d->pair0, d->ctx_pairs);
+    COTR_CHECK(d->q_rows >= 1, "cotr_test_attention: q has %d rows", d->q_rows);
+    COTR_CHECK(d->ldq > 0 && d->ldq % 8 == 0, "cotr_test_attention: ldq %d is not a positive multiple of 8", d->ldq);
+    COTR_CHECK(d->q_col0 >= 0 && d->q_col0 % 8 == 0 && (int64_t)d->q_col0 + kDModel <= d->ldq,
+               "cotr_test_attention: q columns %d .. %d do not fit ldq %d (q_col0 must be a multiple of 8)", d->q_col0,
+               d->q_col0 + kDModel - 1, d->ldq);
+    COTR_CHECK(d->key_split >= 0 && d->key_split <= 2 && (d->path == 0 || d->key_split == 0),
+               "cotr_test_attention: key split %d (0 = launch rule, 1 or 2 on path 0)", d->key_split);
+    COTR_CHECK(d->n_tiles >= 0, "cotr_test_attention: n_tiles %d", d->n_tiles);
+    std::vector<int4> tiles((size_t)d->n_tiles);
+    if (d->n_tiles > 0) {
+        COTR_CHECK(tiles_host, "cotr_test_attention: n_tiles %d without a tile table", d->n_tiles);
+        const int cap = d->path == 0 ? kAttnTcTileRows : kAttnSimtTileRows;
+        for (int i = 0; i < d->n_tiles; ++i) {
+            const int pair = tiles_host[3 * i], row0 = tiles_host[3 * i + 1], rows = tiles_host[3 * i + 2];
+            COTR_CHECK(rows >= 1 && rows <= cap, "cotr_test_attention: tile %d has %d rows (1 .. %d on path %d)", i, rows, cap, d->path);
+            COTR_CHECK(row0 >= 0 && (int64_t)row0 + rows <= d->q_rows, "cotr_test_attention: rows %d .. %d of tile %d fall outside q (%d rows)",
+                       row0, row0 + rows - 1, i, d->q_rows);
+            COTR_CHECK(pair >= 0 && (int64_t)d->pair0 + pair < d->ctx_pairs, "cotr_test_attention: tile %d reads pair %d + %d of %d",
+                       i, d->pair0, pair, d->ctx_pairs);
+            tiles[i] = make_int4(pair, row0, rows, 0);
+        }
+    } else {
+        COTR_CHECK(d->nq >= 1 && d->npairs >= 1, "cotr_test_attention: nq %d, npairs %d", d->nq, d->npairs);
+        COTR_CHECK((int64_t)d->pair0 + d->npairs <= d->ctx_pairs, "cotr_test_attention: pairs %d .. %d of %d", d->pair0,
+                   d->pair0 + d->npairs - 1, d->ctx_pairs);
+        COTR_CHECK((int64_t)d->nq * d->npairs <= d->q_rows, "cotr_test_attention: %d x %d rows, q has %d", d->npairs, d->nq, d->q_rows);
+    }
+
+    DevAllocs mem;
+    TmpSplit q16, o16, k16, v16, vt16, kv16;
+    const size_t kv_rows = (size_t)d->ctx_pairs * kTokens, kv_ld = (size_t)d->slots * kDModel;
+    if (q16.from_f32(q_dev, (size_t)d->q_rows * d->ldq) || o16.from_f32(out_dev, (size_t)d->q_rows * kDModel)) return 1;
+    AttnParams a{};
+    a.q = offset(cs(q16.t), (size_t)d->q_col0); a.ldq = d->ldq;
+    a.out = o16.t; a.ldo = kDModel;
+    a.nq = d->nq; a.npairs = d->npairs; a.pair0 = d->pair0;
+    if (d->operands == 1) {
+        float* kv = nullptr;
+        void* wtc = nullptr;
+        float scale = 1.f;
+        unsigned char* img = nullptr;
+        const size_t img_bytes = (size_t)d->ctx_pairs * d->slots * kHeads * kAttnHeadImgBytes;
+        const std::vector<float> eye = identity(2 * kDModel);
+        if (mem.alloc((void**)&kv, kv_rows * 2 * kDModel * sizeof(float)) || mem.alloc((void**)&img, img_bytes) ||
+            upload_tc_weight(mem, eye.data(), 2 * kDModel, 2 * kDModel, &wtc, &scale)) return 1;
+        COTR_CHECK_CUDA(cudaMemcpy2D(kv, 2 * kDModel * sizeof(float), k_dev + (size_t)d->slot * kDModel, kv_ld * sizeof(float),
+                                     kDModel * sizeof(float), kv_rows, cudaMemcpyDeviceToDevice));
+        COTR_CHECK_CUDA(cudaMemcpy2D(kv + kDModel, 2 * kDModel * sizeof(float), v_dev + (size_t)d->slot * kDModel, kv_ld * sizeof(float),
+                                     kDModel * sizeof(float), kv_rows, cudaMemcpyDeviceToDevice));
+        COTR_CHECK_CUDA(cudaMemset(img, 0xFF, img_bytes));
+        if (kv16.from_f32(kv, kv_rows * 2 * kDModel)) return 1;
         GemmParams p;
         memset(&p, 0, sizeof(p));
-        p.M = npairs * kTokens; p.N = kDModel; p.K = kDModel;
-        p.a = cs(v16.t); p.a_mode = A_ROWMAJOR; p.lda = kDModel;
-        p.Wt = ed; p.acc_scale = 1.f; p.add_period = 1;
-        p.remap = 1; p.blk_map[0] = -1; p.vt = vt16.t; p.n_vt = 1; p.ldc = kDModel;
-        const int rc = launch_gemm_simt(p, 0);
-        cudaDeviceSynchronize();
-        cudaFree(ed);
-        if (rc) return rc;
+        p.M = (int)kv_rows; p.N = 2 * kDModel; p.K = 2 * kDModel;
+        p.a = cs(kv16.t); p.a_mode = A_ROWMAJOR; p.lda = 2 * kDModel;
+        p.Wtc = wtc; p.acc_scale = scale; p.add_period = 1;
+        p.remap = 1; p.blk_map[0] = -1000 - d->slot; p.blk_map[1] = -(d->slot + 1); p.n_vt = d->slots; p.kv_img = img; p.ldc = 2 * kDModel;
+        if (launch_gemm_tc(p, 0)) return 1;
+        a.kv_img = img + (size_t)d->slot * kHeads * kAttnHeadImgBytes;
+        a.img_pair_stride = (size_t)d->slots * kHeads * kAttnHeadImgBytes;
+    } else {
+        float* wd = nullptr;
+        const std::vector<float> eye = identity(kDModel);
+        if (k16.from_f32(k_dev, kv_rows * kv_ld) || v16.from_f32(v_dev, kv_rows * kv_ld) || vt16.empty(kv_rows * kv_ld) ||
+            mem.upload((void**)&wd, eye.data(), eye.size() * sizeof(float))) return 1;
+        COTR_CHECK_CUDA(cudaMemset(vt16.t.hi, 0xFF, (size_t)(vt16.t.lo - vt16.t.hi) * 2 * sizeof(__half)));
+        GemmParams p;     // transpose V of the slot with an identity "GEMM" stored through the transposed-block epilogue
+        memset(&p, 0, sizeof(p));
+        p.M = (int)kv_rows; p.N = kDModel; p.K = kDModel;
+        p.a = offset(cs(v16.t), (size_t)d->slot * kDModel); p.a_mode = A_ROWMAJOR; p.lda = (int)kv_ld;
+        p.Wt = wd; p.acc_scale = 1.f; p.add_period = 1;
+        p.remap = 1; p.blk_map[0] = -(d->slot + 1); p.vt = vt16.t; p.n_vt = d->slots; p.ldc = kDModel;
+        if (launch_gemm_simt(p, 0)) return 1;
+        a.k = offset(cs(k16.t), (size_t)d->slot * kDModel); a.ldk = (int)kv_ld;
+        a.vt = offset(cs(vt16.t), (size_t)d->slot * kVtLayer); a.vt_pair_stride = (size_t)d->slots * kVtLayer;
     }
-    AttnParams a{};
-    a.q = cs(q16.t); a.ldq = kDModel; a.k = cs(k16.t); a.ldk = kDModel;
-    a.vt = cs(vt16.t); a.vt_pair_stride = kVtLayer;
-    a.out = o16.t; a.ldo = kDModel; a.nq = nq; a.npairs = npairs; a.pair0 = 0;
-    int rc = path == 0 ? launch_attention_tc(a, 0) : launch_attention_simt(a, 0);
-    if (!rc) rc = launch_split16_to_f32(cs(o16.t), out_dev, qn, 0);
-    cudaError_t e = cudaDeviceSynchronize();
+    if (d->n_tiles > 0) {
+        int4* tab = nullptr;
+        if (mem.upload((void**)&tab, tiles.data(), tiles.size() * sizeof(int4))) return 1;
+        a.tiles = tab; a.n_tiles = d->n_tiles;
+    }
+    int rc;
+    if (d->path == 1) rc = launch_attention_simt(a, 0);
+    else rc = d->key_split ? launch_attention_tc_split(a, d->key_split, 0) : launch_attention_tc(a, 0);
+    if (!rc) rc = launch_split16_to_f32(cs(o16.t), out_dev, (size_t)d->q_rows * kDModel, 0);
+    const cudaError_t e = cudaDeviceSynchronize();
     if (rc) return rc;
     COTR_CHECK(e == cudaSuccess, "cotr_test_attention: kernel failed: %s", cudaGetErrorString(e));
+    return 0;
+}
+
+// The fused feed-forward launch on its own; `out` (or x, in place) is converted in before the launch, so the rows >= M
+// come back as they were passed.
+int cotr_test_mlp(const cotr_test_mlp_desc* d, const float* x_dev, const float* w1_host, const float* b1_dev,
+                  const float* w2_host, const float* b2_dev, const float* g_dev, const float* be_dev,
+                  const float* g2_dev, const float* be2_dev, float* out_dev) {
+    COTR_CHECK(d && x_dev && w1_host && b1_dev && w2_host && b2_dev && g_dev && be_dev && out_dev, "cotr_test_mlp: null argument");
+    COTR_CHECK((g2_dev == nullptr) == (be2_dev == nullptr), "cotr_test_mlp: g2 and be2 go together");
+    COTR_CHECK(d->M >= 1 && d->rows >= d->M, "cotr_test_mlp: M %d of %d rows", d->M, d->rows);
+    COTR_CHECK(d->split == 0 || d->split == 4 || d->split == 8, "cotr_test_mlp: split %d (0 = launch rule, 4 or 8)", d->split);
+    const size_t n = (size_t)d->rows * kDModel;
+    DevAllocs mem;
+    TmpSplit x16, o16;
+    if (x16.from_f32(x_dev, n) || (!d->in_place && o16.from_f32(out_dev, n))) return 1;
+    MlpParams p;
+    memset(&p, 0, sizeof(p));
+    void *w1 = nullptr, *w2 = nullptr;
+    if (upload_tc_weight(mem, w1_host, kFF, kDModel, &w1, &p.w1_scale) || upload_tc_weight(mem, w2_host, kDModel, kFF, &w2, &p.w2_scale)) return 1;
+    p.M = d->M; p.x = cs(x16.t); p.out = d->in_place ? x16.t : o16.t;
+    p.w1 = w1; p.b1 = b1_dev; p.w2 = w2; p.b2 = b2_dev;
+    p.g = g_dev; p.be = be_dev; p.g2 = g2_dev; p.be2 = be2_dev;
+    int rc = d->split ? launch_mlp_tc_split(p, d->split, 0) : launch_mlp_tc(p, 0);
+    if (!rc) rc = launch_split16_to_f32(cs(p.out), out_dev, n, 0);
+    const cudaError_t e = cudaDeviceSynchronize();
+    if (rc) return rc;
+    COTR_CHECK(e == cudaSuccess, "cotr_test_mlp: kernel failed: %s", cudaGetErrorString(e));
+    return 0;
+}
+
+int cotr_test_rowwise(int op, int rows, const float* in_dev, const float* g1_dev, const float* b1_dev,
+                      const float* g2_dev, const float* b2_dev, float* out_dev) {
+    COTR_CHECK(in_dev && out_dev && rows >= 1, "cotr_test_rowwise: null argument or %d rows", rows);
+    COTR_CHECK(op >= 0 && op <= 3, "cotr_test_rowwise: op %d (0 LayerNorm, 1 fp32 LayerNorm, 2 two LayerNorms, 3 query encoding)", op);
+    COTR_CHECK(op == 3 || (g1_dev && b1_dev), "cotr_test_rowwise: op %d needs g1 / b1", op);
+    COTR_CHECK(op != 2 || (g2_dev && b2_dev), "cotr_test_rowwise: op 2 needs g2 / b2");
+    const size_t n = (size_t)rows * kDModel;
+    TmpSplit x16, o16;
+    if (o16.empty(n) || ((op == 0 || op == 2) && x16.from_f32(in_dev, n))) return 1;
+    int rc;
+    switch (op) {
+        case 0: rc = launch_layernorm(cs(x16.t), g1_dev, b1_dev, o16.t, rows, 0); break;
+        case 1: rc = launch_layernorm_f32(in_dev, g1_dev, b1_dev, o16.t, rows, 0); break;
+        case 2: rc = launch_layernorm_twice(cs(x16.t), g1_dev, b1_dev, g2_dev, b2_dev, o16.t, rows, 0); break;
+        default: rc = launch_query_encode(in_dev, o16.t, rows, 0); break;
+    }
+    if (!rc) rc = launch_split16_to_f32(cs(o16.t), out_dev, n, 0);
+    const cudaError_t e = cudaDeviceSynchronize();
+    if (rc) return rc;
+    COTR_CHECK(e == cudaSuccess, "cotr_test_rowwise: kernel failed: %s", cudaGetErrorString(e));
     return 0;
 }
 

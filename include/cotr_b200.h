@@ -270,9 +270,39 @@ typedef struct cotr_test_gemm_desc {
 int cotr_test_gemm(const cotr_test_gemm_desc* d, const float* A_dev, const float* w_host, const float* bias_dev,
                    const float* addmat_dev, const float* residual_dev, const float* ln_gamma_dev,
                    const float* ln_beta_dev, float* out_dev, float* part_out_dev /* [M][16][2] or NULL */);
-/* out[(p*nq+i), h*32+d] = softmax(q k^T) v per head; q (npairs*nq,256), k/v (npairs*512,256), all DEVICE, ld 256. */
-int cotr_test_attention(int path, const float* q_dev, const float* k_dev, const float* v_dev, float* out_dev,
-                        int nq, int npairs);
+typedef struct cotr_test_attention_desc {
+    int32_t path;                 /* 0 = wgmma (attention_tc.cu), 1 = fp32 SIMT (attention_simt.cu)                */
+    int32_t nq, npairs;           /* uniform layout: local pair p owns q / out rows p*nq .. p*nq+nq-1             */
+    int32_t operands;             /* 0: K row-major, V transposed (fp32 SIMT schedule); 1: attention operand images,
+                                     written by the tensor-core K/V projection epilogue (tensor-core schedule)        */
+    int32_t slots, slot;          /* k / v hold `slots` layers side by side, as a context does; the launch reads `slot` */
+    int32_t ctx_pairs, pair0;     /* k / v hold ctx_pairs pairs; the launch reads pairs pair0 ..                       */
+    int32_t q_rows, ldq, q_col0;  /* q (q_rows, ldq), the launch reads its columns q_col0 .. q_col0+255; out (q_rows,256) */
+    int32_t n_tiles;              /* > 0: tiles_host holds n_tiles (pair, first row, row count) triples (ragged decode) */
+    int32_t key_split;            /* path 0: 0 = the launch rule, 1 or 2 = that key split                             */
+    int32_t reserved;
+} cotr_test_attention_desc;
+/* out[r, h*32+d] = softmax(q k^T) v per head for the rows the launch owns; every other row of out is left as it was
+ * passed.  q (q_rows,ldq), k / v (ctx_pairs*512, slots*256), out (q_rows,256): fp32 DEVICE; tiles_host int32 HOST or NULL.
+ * Every argument is checked before anything is launched. */
+int cotr_test_attention(const cotr_test_attention_desc* d, const float* q_dev, const float* k_dev, const float* v_dev,
+                        float* out_dev, const int32_t* tiles_host);
+typedef struct cotr_test_mlp_desc {
+    int32_t M;                    /* rows of the launch                                                             */
+    int32_t rows;                 /* rows of x and out (>= M)                                                        */
+    int32_t split;                /* 0 = the launch rule, 4 or 8 = CTAs per row tile                                  */
+    int32_t in_place;             /* 1: the launch writes into x (out == x, as the decoder runs it); out receives x after */
+} cotr_test_mlp_desc;
+/* The fused feed-forward block (mlp_tc.cu): out = LN(x + relu(x W1^T + b1) W2^T + b2) [then LN2 when g2 / be2 are given]
+ * on rows < M; rows >= M of out are left as they were passed.  x / out (rows,256), b1 (1024), b2 / g / be / g2 / be2 (256):
+ * fp32 DEVICE; w1 [1024,256], w2 [256,1024]: fp32 HOST. */
+int cotr_test_mlp(const cotr_test_mlp_desc* d, const float* x_dev, const float* w1_host, const float* b1_dev,
+                  const float* w2_host, const float* b2_dev, const float* g_dev, const float* be_dev,
+                  const float* g2_dev, const float* be2_dev, float* out_dev);
+/* Row kernels: op 0 LayerNorm of a split16 input, 1 LayerNorm of an fp32 input, 2 LN2(LN1(x)) (g2 / b2),
+ * 3 lin_sine query encoding of (rows,2) points in [0,1] (in; g1 .. b2 unused).  in (rows,256), out (rows,256): DEVICE. */
+int cotr_test_rowwise(int op, int rows, const float* in_dev, const float* g1_dev, const float* b1_dev,
+                      const float* g2_dev, const float* b2_dev, float* out_dev);
 /* out[(p*nq+i), j] = head-averaged softmax(q k^T) (the maps of cotr_decode_attention); q (npairs*nq,256), k (npairs*512,256),
  * out (npairs,nq,512), all DEVICE.  Path 0 reads k through the attention operand images, path 1 row-major. */
 int cotr_test_attention_weights(int path, const float* q_dev, const float* k_dev, float* out_dev, int nq, int npairs);
