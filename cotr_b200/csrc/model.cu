@@ -42,7 +42,9 @@ struct DevConv {
 
 struct DevLinear {
     float* w = nullptr;    // [N][K]
-    void* wtc = nullptr;
+    void* wtc_plain = nullptr;       // tensor-core image of W (explicit-LayerNorm schedule)
+    float wtc_plain_scale = 1.f;
+    void* wtc = nullptr;             // image of the deferred-LayerNorm schedule: wtc_plain unless built by make_linear_ln
     float wtc_scale = 1.f;
     float* b = nullptr;    // [N] or null
     int n = 0, k = 0;
@@ -50,8 +52,6 @@ struct DevLinear {
     // cs its column sums and b_tc = beta W^T + b; w / b stay the checkpoint's values for the fp32 SIMT path.
     float* cs = nullptr;
     float* b_tc = nullptr;
-    void* wtc_plain = nullptr;       // tensor-core image of the un-folded W (explicit-LayerNorm schedule on the tensor-core path)
-    float wtc_plain_scale = 1.f;
 };
 
 struct Block {
@@ -97,6 +97,39 @@ struct Workspace {
     size_t img_stage_elems = 0, q_stage_elems = 0;
 };
 
+// A host table that reaches the device with one asynchronous copy per call, staged through pinned memory.  `copied` is
+// recorded after each copy out of `stage`; the host rewrites `stage` only once that copy has completed, which it has
+// long done unless the host runs a whole call ahead of the device.
+template <class T>
+struct PinnedTable {
+    T* dev = nullptr;
+    T* stage = nullptr;
+    size_t cap = 0;
+    cudaEvent_t copied = nullptr;
+    ~PinnedTable() {
+        if (dev) cudaFree(dev);
+        if (stage) cudaFreeHost(stage);
+        if (copied) cudaEventDestroy(copied);
+    }
+    int upload(const T* src, size_t n, cudaStream_t s) {
+        if (n > cap) {
+            COTR_CHECK_CUDA(cudaDeviceSynchronize());
+            cap = 0;      // a failed allocation below leaves no capacity behind, so the next call allocates again
+            if (dev) { cudaFree(dev); dev = nullptr; }
+            if (stage) { cudaFreeHost(stage); stage = nullptr; }
+            COTR_CHECK_CUDA(cudaMalloc((void**)&dev, n * sizeof(T)));
+            COTR_CHECK_CUDA(cudaMallocHost((void**)&stage, n * sizeof(T)));
+            cap = n;
+        }
+        if (!copied) COTR_CHECK_CUDA(cudaEventCreateWithFlags(&copied, cudaEventDisableTiming));
+        COTR_CHECK_CUDA(cudaEventSynchronize(copied));
+        memcpy(stage, src, n * sizeof(T));
+        COTR_CHECK_CUDA(cudaMemcpyAsync(dev, stage, n * sizeof(T), cudaMemcpyHostToDevice, s));
+        COTR_CHECK_CUDA(cudaEventRecord(copied, s));
+        return 0;
+    }
+};
+
 }  // namespace
 }  // namespace cotr
 
@@ -140,17 +173,8 @@ struct cotr_model {
     std::map<long long, cudaGraphExec_t> graphs;
     std::map<long long, int> graph_launches;
     std::set<long long> shapes_seen;
-    // cotr_encode_context_pairs: the caller's (B,2) image table, staged through pinned memory.  pair_copied is recorded
-    // after each copy out of pair_stage; the host rewrites pair_stage only once that copy has completed.
-    int* pair_tab = nullptr;
-    int* pair_stage = nullptr;
-    int pair_cap = 0;
-    cudaEvent_t pair_copied = nullptr;
-    // cotr_decode_ragged: the attention tile tables of all chunks of a call (AttnParams::tiles), staged the same way
-    int4* tile_tab = nullptr;
-    int4* tile_stage = nullptr;
-    size_t tile_cap = 0;
-    cudaEvent_t tile_copied = nullptr;
+    cotr::PinnedTable<int> pair_tab;     // cotr_encode_context_pairs: the caller's (B,2) image table
+    cotr::PinnedTable<int4> tile_tab;    // cotr_decode_ragged: the attention tile tables of all chunks of a call (AttnParams::tiles)
     cotr::Preprocessor* pre = nullptr;         // device-side crop / resize / normalise (cotr_preprocess)
     cotr::FlowMerger* merger = nullptr;        // device-side tail of the dense first guess (cotr_flow_tile_merge)
     bool prof_on = false;
@@ -211,34 +235,47 @@ int upload_tc(cotr_model* m, const std::vector<float>& w, int N, int K, void** d
 int make_linear(cotr_model* m, const std::vector<float>& w, const std::vector<float>* b, int N, int K, DevLinear* out) {
     out->n = N; out->k = K;
     if (upload(m, w, &out->w)) return 1;
-    if (upload_tc(m, w, N, K, &out->wtc, &out->wtc_scale)) return 1;
+    if (upload_tc(m, w, N, K, &out->wtc_plain, &out->wtc_plain_scale)) return 1;
+    out->wtc = out->wtc_plain; out->wtc_scale = out->wtc_plain_scale;
     if (b) { if (upload(m, *b, &out->b)) return 1; }
     return 0;
 }
 
-// Linear layer whose input is a deferred LayerNorm (gamma, beta): tensor-core image of W diag(gamma), its column sums
-// and the folded bias beta W^T + b (see GemmParams::a_ln_cs).
+// A linear layer W [N][K] + b (b may be null) whose input is a deferred LayerNorm (gamma, beta): the tensor-core GEMM
+// multiplies by w = W diag(gamma), its epilogue takes the column sums cs of w and the folded bias b = beta W^T + b
+// (see GemmParams::a_ln_cs).  The sums are taken in double.
+struct LnFold {
+    std::vector<float> w, cs, b;
+};
+LnFold fold_ln(const float* w, const float* b, int N, int K, const float* gamma, const float* beta) {
+    LnFold f;
+    f.w.resize((size_t)N * K); f.cs.resize(N); f.b.resize(N);
+    for (int n = 0; n < N; ++n) {
+        double s = 0.0, c = b ? (double)b[n] : 0.0;
+        for (int k = 0; k < K; ++k) {
+            const float v = w[(size_t)n * K + k] * gamma[k];
+            f.w[(size_t)n * K + k] = v;
+            s += (double)v;
+            c += (double)w[(size_t)n * K + k] * (double)beta[k];
+        }
+        f.cs[n] = (float)s;
+        f.b[n] = (float)c;
+    }
+    return f;
+}
+
+// Linear layer whose input is a deferred LayerNorm (gamma, beta): wtc holds the folded image (fold_ln), wtc_plain the
+// image of W itself.
 int make_linear_ln(cotr_model* m, const std::vector<float>& w, const std::vector<float>* b, int N, int K,
                    const float* gamma, const float* beta, DevLinear* out, std::vector<float>* folded_bias = nullptr) {
     out->n = N; out->k = K;
     if (upload(m, w, &out->w)) return 1;
     if (b) { if (upload(m, *b, &out->b)) return 1; }
-    std::vector<float> wg((size_t)N * K), cs(N), cb(N);
-    for (int n = 0; n < N; ++n) {
-        double s = 0.0, c = b ? (double)(*b)[n] : 0.0;
-        for (int k = 0; k < K; ++k) {
-            const float v = w[(size_t)n * K + k] * gamma[k];
-            wg[(size_t)n * K + k] = v;
-            s += (double)v;
-            c += (double)w[(size_t)n * K + k] * (double)beta[k];
-        }
-        cs[n] = (float)s;
-        cb[n] = (float)c;
-    }
-    if (upload_tc(m, wg, N, K, &out->wtc, &out->wtc_scale)) return 1;
+    const LnFold f = fold_ln(w.data(), b ? b->data() : nullptr, N, K, gamma, beta);
+    if (upload_tc(m, f.w, N, K, &out->wtc, &out->wtc_scale)) return 1;
     if (upload_tc(m, w, N, K, &out->wtc_plain, &out->wtc_plain_scale)) return 1;
-    if (upload(m, cs, &out->cs) || upload(m, cb, &out->b_tc)) return 1;
-    if (folded_bias) *folded_bias = cb;
+    if (upload(m, f.cs, &out->cs) || upload(m, f.b, &out->b_tc)) return 1;
+    if (folded_bias) *folded_bias = f.b;
     return 0;
 }
 
@@ -360,6 +397,27 @@ GemmParams gemm_base(int M, int N, int K, CSplit16 A, int lda, const float* W, c
     return p;
 }
 
+// GEMM of linear layer L; folded: with the deferred-LayerNorm schedule's weight image (DevLinear::wtc)
+GemmParams gemm_linear(const DevLinear& L, bool folded, int M, CSplit16 A, int lda, Split16 out, int ldc) {
+    if (folded) return gemm_base(M, L.n, L.k, A, lda, L.w, L.wtc, L.wtc_scale, out, ldc);
+    return gemm_base(M, L.n, L.k, A, lda, L.w, L.wtc_plain, L.wtc_plain_scale, out, ldc);
+}
+
+// Redirects the 256-column blocks of a key / value projection (GemmParams::remap): the blocks before kv0 keep their
+// columns, then come `slots` (key, value) block pairs.  The keys of slot l go to columns k_col0 + 256 l of the output,
+// or into slot l's attention operand images when kv_img is set; the values go transposed to slot l of vt, or into the
+// images.
+void redirect_kv(GemmParams& p, int kv0, int slots, int k_col0, Split16 vt, unsigned char* kv_img) {
+    p.remap = 1;
+    for (int b = 0; b < kv0; ++b) p.blk_map[b] = b * kDModel;
+    for (int l = 0; l < slots; ++l) {
+        p.blk_map[kv0 + 2 * l] = kv_img ? -1000 - l : k_col0 + l * kDModel;
+        p.blk_map[kv0 + 2 * l + 1] = -(l + 1);
+    }
+    p.vt = vt; p.n_vt = slots;
+    p.kv_img = kv_img;
+}
+
 int launch_tc(const Run& r, const GemmParams& p) {
     LaunchScope scope(r, K_GEMM_TC, p.M, p.N, p.K);
     return launch_gemm_tc(p, r.s);
@@ -403,8 +461,7 @@ int run_gemm(const Run& r, GemmParams p, float* ln_scratch) {
 int run_linear(const Run& r, const DevLinear& L, int M, CSplit16 A, int lda, Split16 out, int ldc, bool relu,
                CSplit16 residual = CSplit16{nullptr, nullptr}, int ldr = 0, const float* ln_g = nullptr,
                const float* ln_b = nullptr, float* ln_scratch = nullptr) {
-    // explicit-LayerNorm schedule: layers that also exist in a gamma-folded form use their plain image here
-    GemmParams p = gemm_base(M, L.n, L.k, A, lda, L.w, L.wtc_plain ? L.wtc_plain : L.wtc, L.wtc_plain ? L.wtc_plain_scale : L.wtc_scale, out, ldc);
+    GemmParams p = gemm_linear(L, false, M, A, lda, out, ldc);
     p.bias = L.b;
     p.relu = relu ? 1 : 0;
     p.res = residual; p.ldr = ldr;
@@ -419,8 +476,8 @@ int run_mlp(const Run& r, const DevLinear& l1, const DevLinear& l2, int M, CSpli
     MlpParams p;
     memset(&p, 0, sizeof(p));
     p.M = M; p.x = x; p.out = out;
-    p.w1 = l1.wtc_plain ? l1.wtc_plain : l1.wtc; p.w1_scale = l1.wtc_plain ? l1.wtc_plain_scale : l1.wtc_scale; p.b1 = l1.b;
-    p.w2 = l2.wtc_plain ? l2.wtc_plain : l2.wtc; p.w2_scale = l2.wtc_plain ? l2.wtc_plain_scale : l2.wtc_scale; p.b2 = l2.b;
+    p.w1 = l1.wtc_plain; p.w1_scale = l1.wtc_plain_scale; p.b1 = l1.b;
+    p.w2 = l2.wtc_plain; p.w2_scale = l2.wtc_plain_scale; p.b2 = l2.b;
     p.g = g; p.be = b; p.g2 = g2; p.be2 = b2;
     LaunchScope scope(r, K_GEMM_MLP, M, kFF, 2 * kDModel);
     return launch_mlp_tc(p, r.s);
@@ -433,7 +490,7 @@ int run_mlp(const Run& r, const DevLinear& l1, const DevLinear& l2, int M, CSpli
 int run_linear_dln(const Run& r, const DevLinear& L, int M, CSplit16 A, int lda, Split16 out, int ldc, bool relu,
                    const float2* a_part, float2* part_out, CSplit16 residual = CSplit16{nullptr, nullptr}, int ldr = 0,
                    const float2* res_part = nullptr, const float* res_g = nullptr, const float* res_b = nullptr) {
-    GemmParams p = gemm_base(M, L.n, L.k, A, lda, L.w, L.wtc, L.wtc_scale, out, ldc);
+    GemmParams p = gemm_linear(L, true, M, A, lda, out, ldc);
     p.bias = a_part ? L.b_tc : L.b;
     p.relu = relu ? 1 : 0;
     p.res = residual; p.ldr = ldr;
@@ -462,13 +519,6 @@ int run_conv(const Run& r, const DevConv& c, int n_img, CSplit16 in, int H, int 
     return run_gemm(r, p, nullptr);
 }
 
-int run_attention(const Run& r, const AttnParams& p) {
-    // recorded as M = query rows, N = 512 keys, K = 32 x 8 heads
-    LaunchScope scope(r, r.m->gemm_path == 0 ? K_ATTN_TC : K_ATTN_SIMT, p.nq * p.npairs, kTokens, kDModel);
-    if (r.m->gemm_path != 0) return launch_attention_simt(p, r.s);
-    return launch_attention_tc(p, r.s);
-}
-
 // The attention tiles of one ragged decode chunk (cotr_decode_ragged): a device table of n_tc tensor-core tiles
 // (kAttnTcTileRows rows of a pair with >= kAttnTcMinRows rows in the chunk) followed by n_simt SIMT tiles
 // (kAttnSimtTileRows rows: the other pairs, or every pair on the fp32 SIMT path), see AttnParams::tiles.
@@ -478,16 +528,23 @@ struct ChunkTiles {
     int rows_tc = 0, rows_simt = 0;
 };
 
-// One launch per kind of tile present; the two launches write disjoint rows of the output.
-int run_attention_tiles(const Run& r, AttnParams a, const ChunkTiles& t) {
-    if (t.n_tc > 0) {
-        a.tiles = t.tab; a.n_tiles = t.n_tc;
-        LaunchScope scope(r, K_ATTN_TC, t.rows_tc, kTokens, kDModel);
+// Recorded as M = query rows, N = 512 keys, K = 32 x 8 heads.  Without tiles: one launch over nq rows of each of npairs
+// pairs.  With the tiles of a ragged chunk: one launch per kind of tile present; the two launches write disjoint rows
+// of the output.
+int run_attention(const Run& r, AttnParams a, const ChunkTiles* t = nullptr) {
+    if (!t) {
+        LaunchScope scope(r, r.m->gemm_path == 0 ? K_ATTN_TC : K_ATTN_SIMT, a.nq * a.npairs, kTokens, kDModel);
+        if (r.m->gemm_path != 0) return launch_attention_simt(a, r.s);
+        return launch_attention_tc(a, r.s);
+    }
+    if (t->n_tc > 0) {
+        a.tiles = t->tab; a.n_tiles = t->n_tc;
+        LaunchScope scope(r, K_ATTN_TC, t->rows_tc, kTokens, kDModel);
         if (launch_attention_tc(a, r.s)) return 1;
     }
-    if (t.n_simt > 0) {
-        a.tiles = t.tab + t.n_tc; a.n_tiles = t.n_simt;
-        LaunchScope scope(r, K_ATTN_SIMT, t.rows_simt, kTokens, kDModel);
+    if (t->n_simt > 0) {
+        a.tiles = t->tab + t->n_tc; a.n_tiles = t->n_simt;
+        LaunchScope scope(r, K_ATTN_SIMT, t->rows_simt, kTokens, kDModel);
         if (launch_attention_simt(a, r.s)) return 1;
     }
     return 0;
@@ -507,6 +564,16 @@ struct AttnMaps {
     }
     AttnMaps at(size_t elems) const { AttnMaps a = *this; if (a.base) a.base += elems; return a; }
 };
+
+// The maps of a call over B pairs with `rows` query rows each, into the caller's (n_sel, B, rows, 512) buffer
+AttnMaps attn_maps(int layer_mask, float* attn_dev, int B, size_t rows) {
+    AttnMaps maps;
+    maps.mask = (unsigned)layer_mask;
+    maps.base = attn_dev;
+    maps.layer_stride = (size_t)B * rows * kTokens;
+    maps.pair_stride = rows * kTokens;
+    return maps;
+}
 
 // The maps of one layer from the operands its attention launch `a` just read (attention_weights.cu); recorded like the
 // attention launch (M = query rows, N = 512 keys, K = 32 x 8 heads).
@@ -532,16 +599,6 @@ constexpr size_t kBigElems = 64 * 64 * 256;        // largest block input / outp
 constexpr size_t kT1Elems = 64 * 64 * 128;         // largest conv1 output per image (layer2.0)
 constexpr size_t kT2Elems = 64 * 64 * 64;          // largest conv2 output per image (layer1)
 
-size_t encode_ws_elems(int B) {
-    const size_t img = 2 * (size_t)B;
-    const size_t tok = (size_t)B * kTokens;
-    return img * (kStemCanvasElems + kStemElems + 3 * kBigElems + kT1Elems + kT2Elems) + tok * (kDModel * 4 + 2 * kDModel + kFF) +
-           (size_t)B * kVtLayer + tok * kDModel /* fp32 LN scratch */ + tok * 64 /* row statistics */;
-}
-size_t decode_ws_elems(int rows) {
-    return (size_t)rows * (kDModel * 8 + kQpCols + kFF) + (size_t)rows * kDModel /* fp32 LN scratch */ + (size_t)rows * 64 /* row statistics */;
-}
-
 // split16 buffer of `elems` elements: one allocation, hi plane first (elems is always a multiple of 8)
 int ws_alloc(Split16* t, size_t elems) {
     __half* base = nullptr;
@@ -556,6 +613,92 @@ int ws_alloc_f32(float** p, size_t elems) {
     return 0;
 }
 void ws_free_f32(float** p) { if (*p) { cudaFree(*p); *p = nullptr; } }
+
+// One workspace buffer: a split16 tensor (allocated as ws_alloc does) or a plain device array, and its size.
+struct WsBuf {
+    Split16* split;
+    void** raw;
+    size_t bytes;
+};
+WsBuf ws_split(Split16* t, size_t elems) { return {t, nullptr, elems * 2 * sizeof(__half)}; }
+template <class T>
+WsBuf ws_raw(T** p, size_t elems) { return {nullptr, reinterpret_cast<void**>(p), elems * sizeof(T)}; }
+
+// Every buffer of a section's workspace with its size, listed once: allocation, release and cotr_workspace_bytes all
+// walk these lists.  Encoder: the backbone of 2B images and the transformer of B pairs.
+std::vector<WsBuf> encode_ws_bufs(Workspace& w, int B) {
+    const size_t img = 2 * (size_t)B, tok = (size_t)B * kTokens;
+    return {ws_split(&w.canvas, img * kStemCanvasElems), ws_split(&w.stem, img * kStemElems),
+            ws_split(&w.bx, img * kBigElems), ws_split(&w.by, img * kBigElems), ws_split(&w.bds, img * kBigElems),
+            ws_split(&w.bt1, img * kT1Elems), ws_split(&w.bt2, img * kT2Elems),
+            ws_split(&w.src, tok * kDModel), ws_split(&w.xa, tok * kDModel), ws_split(&w.xb, tok * kDModel),
+            ws_split(&w.qk, tok * 2 * kDModel), ws_split(&w.vt, (size_t)B * kVtLayer), ws_split(&w.ao, tok * kDModel),
+            ws_split(&w.ffh, tok * kFF), ws_raw(&w.ln_tmp, tok * kDModel),
+            ws_raw(&w.enc_st_a, tok * 16), ws_raw(&w.enc_st_b, tok * 16),
+            ws_raw(&w.kvimg, (size_t)B * kHeads * kAttnHeadImgBytes), ws_raw(&w.pair_id, img)};
+}
+// Decoder: `rows` query rows, rounded up to a multiple of 8 (ws_alloc's condition).
+std::vector<WsBuf> decode_ws_bufs(Workspace& w, int rows) {
+    const size_t R = ((size_t)rows + 7) & ~(size_t)7;
+    return {ws_split(&w.qpos, R * kDModel), ws_split(&w.qp, R * kQpCols), ws_split(&w.t, R * kDModel),
+            ws_split(&w.qb, R * kDModel), ws_split(&w.dao, R * kDModel), ws_split(&w.dh, R * kFF),
+            ws_split(&w.hs, R * kDModel), ws_split(&w.hd1, R * kDModel), ws_split(&w.hd2, R * kDModel),
+            ws_split(&w.t2, R * kDModel), ws_raw(&w.dln_tmp, R * kDModel),
+            ws_raw(&w.dec_st_a, R * 16), ws_raw(&w.dec_st_b, R * 16)};
+}
+
+void ws_release(const std::vector<WsBuf>& bufs) {
+    for (const WsBuf& b : bufs) {
+        if (b.split) ws_free(b.split);
+        else if (*b.raw) { cudaFree(*b.raw); *b.raw = nullptr; }
+    }
+}
+int ws_allocate(const std::vector<WsBuf>& bufs) {
+    for (const WsBuf& b : bufs) {
+        void* base = nullptr;
+        COTR_CHECK_CUDA(cudaMalloc(&base, b.bytes));
+        if (b.split) {
+            b.split->hi = static_cast<__half*>(base);
+            b.split->lo = b.split->hi + b.bytes / (2 * sizeof(__half));
+        } else {
+            *b.raw = base;
+        }
+    }
+    return 0;
+}
+size_t ws_bytes(const std::vector<WsBuf>& bufs) {
+    size_t n = 0;
+    for (const WsBuf& b : bufs) n += b.bytes;
+    return n;
+}
+
+// Temporaries of one call (model construction, test hooks), freed on every return (cudaFree waits for the work queued
+// on them).
+struct DevAllocs {
+    std::vector<void*> ptrs;
+    ~DevAllocs() { for (void* p : ptrs) cudaFree(p); }
+    int alloc(void** out, size_t bytes) {
+        COTR_CHECK_CUDA(cudaMalloc(out, bytes));
+        ptrs.push_back(*out);
+        return 0;
+    }
+    int upload(void** out, const void* host, size_t bytes) {
+        if (alloc(out, bytes)) return 1;
+        COTR_CHECK_CUDA(cudaMemcpy(*out, host, bytes, cudaMemcpyHostToDevice));
+        return 0;
+    }
+};
+
+struct TmpSplit {
+    Split16 t = kNoSplit;
+    ~TmpSplit() { ws_free(&t); }
+    int from_f32(const float* src, size_t n) {
+        const size_t padded = (n + 7) & ~(size_t)7;
+        if (ws_alloc(&t, padded)) return 1;
+        return launch_f32_to_split16(src, t, n, 0);
+    }
+    int empty(size_t n) { return ws_alloc(&t, (n + 7) & ~(size_t)7); }
+};
 
 // Schedule selection.
 // Deferred LayerNorm (no LayerNorm launches; consumers normalise on the fly) removes 12 launches from the encoder and
@@ -603,30 +746,15 @@ int ensure_encode_ws(cotr_model* m, int B) {
     COTR_CHECK_CUDA(cudaDeviceSynchronize());
     drop_graphs(m);
     w.cap_pairs = 0;      // a failed allocation below leaves no capacity behind, so the next call allocates again
-    Split16* bufs[] = {&w.canvas, &w.stem, &w.bx, &w.by, &w.bt1, &w.bt2, &w.bds, &w.src, &w.xa, &w.xb, &w.qk, &w.vt, &w.ao, &w.ffh};
-    for (Split16* b : bufs) ws_free(b);
-    ws_free_f32(&w.ln_tmp);
-    if (w.kvimg) { cudaFree(w.kvimg); w.kvimg = nullptr; }
-    ws_free_f32(reinterpret_cast<float**>(&w.enc_st_a));
-    ws_free_f32(reinterpret_cast<float**>(&w.enc_st_b));
-    const size_t img = 2 * (size_t)B, tok = (size_t)B * kTokens;
-    if (ws_alloc(&w.canvas, img * kStemCanvasElems) || ws_alloc(&w.stem, img * kStemElems) || ws_alloc(&w.bx, img * kBigElems) || ws_alloc(&w.by, img * kBigElems) ||
-        ws_alloc(&w.bds, img * kBigElems) || ws_alloc(&w.bt1, img * kT1Elems) || ws_alloc(&w.bt2, img * kT2Elems) ||
-        ws_alloc(&w.src, tok * kDModel) || ws_alloc(&w.xa, tok * kDModel) || ws_alloc(&w.xb, tok * kDModel) ||
-        ws_alloc(&w.qk, tok * 2 * kDModel) || ws_alloc(&w.vt, (size_t)B * kVtLayer) || ws_alloc(&w.ao, tok * kDModel) ||
-        ws_alloc(&w.ffh, tok * kFF) || ws_alloc_f32(&w.ln_tmp, tok * kDModel) ||
-        ws_alloc_f32(reinterpret_cast<float**>(&w.enc_st_a), tok * 32) || ws_alloc_f32(reinterpret_cast<float**>(&w.enc_st_b), tok * 32))
-        return 1;
-    if (w.pair_id) { cudaFree(w.pair_id); w.pair_id = nullptr; }
+    ws_release(encode_ws_bufs(w, 0));
+    if (ws_allocate(encode_ws_bufs(w, B))) return 1;
     std::vector<int> ident(2 * (size_t)B);
     for (size_t i = 0; i < ident.size(); ++i) ident[i] = (int)i;
-    COTR_CHECK_CUDA(cudaMalloc((void**)&w.pair_id, ident.size() * sizeof(int)));
     COTR_CHECK_CUDA(cudaMemcpy(w.pair_id, ident.data(), ident.size() * sizeof(int), cudaMemcpyHostToDevice));
-    COTR_CHECK_CUDA(cudaMalloc((void**)&w.kvimg, (size_t)B * kHeads * kAttnHeadImgBytes));
     // the 16 pad bytes of every value key group are copied by the bulk TMA: keep them defined
     COTR_CHECK_CUDA(cudaMemset(w.kvimg, 0, (size_t)B * kHeads * kAttnHeadImgBytes));
     // the border of the stem canvas is the convolution's zero padding: written here, never again
-    COTR_CHECK_CUDA(cudaMemset(w.canvas.hi, 0, img * kStemCanvasElems * 2 * sizeof(__half)));
+    COTR_CHECK_CUDA(cudaMemset(w.canvas.hi, 0, 2 * (size_t)B * kStemCanvasElems * 2 * sizeof(__half)));
     w.cap_pairs = B;
     return 0;
 }
@@ -637,18 +765,8 @@ int ensure_decode_ws(cotr_model* m, int rows) {
     COTR_CHECK_CUDA(cudaDeviceSynchronize());
     drop_graphs(m);
     w.cap_rows = 0;       // as in ensure_encode_ws: no stale capacity after a failed allocation
-    Split16* bufs[] = {&w.qpos, &w.qp, &w.t, &w.qb, &w.dao, &w.dh, &w.hs, &w.hd1, &w.hd2, &w.t2};
-    for (Split16* b : bufs) ws_free(b);
-    ws_free_f32(&w.dln_tmp);
-    ws_free_f32(reinterpret_cast<float**>(&w.dec_st_a));
-    ws_free_f32(reinterpret_cast<float**>(&w.dec_st_b));
-    const size_t R = ((size_t)rows + 7) & ~(size_t)7;
-    if (ws_alloc(&w.qpos, R * kDModel) || ws_alloc(&w.qp, R * kQpCols) || ws_alloc(&w.t, R * kDModel) ||
-        ws_alloc(&w.qb, R * kDModel) || ws_alloc(&w.dao, R * kDModel) || ws_alloc(&w.dh, R * kFF) ||
-        ws_alloc(&w.hs, R * kDModel) || ws_alloc(&w.hd1, R * kDModel) || ws_alloc(&w.hd2, R * kDModel) ||
-        ws_alloc(&w.t2, R * kDModel) || ws_alloc_f32(&w.dln_tmp, R * kDModel) ||
-        ws_alloc_f32(reinterpret_cast<float**>(&w.dec_st_a), R * 32) || ws_alloc_f32(reinterpret_cast<float**>(&w.dec_st_b), R * 32))
-        return 1;
+    ws_release(decode_ws_bufs(w, 0));
+    if (ws_allocate(decode_ws_bufs(w, rows))) return 1;
     w.cap_rows = rows;
     return 0;
 }
@@ -716,79 +834,26 @@ int encode_tail(cotr_model* m, CSplit16 feat, const int* pairs, int B, cotr_cont
 
     // transformer.py:143-159 x6 (post-LN).  q = k = x + pos is folded into the constant add_qkv matrix.
     // q | k land row-major in qk [T][512]; v lands transposed in vt [pair][256][512] (what P V needs as its B operand).
-    Split16 xin = w.src;      // layer input
-    if (deferred_ln_enabled(m, T)) {
-        // Tensor-core path: no LayerNorm kernel and no LayerNorm epilogue.  A LayerNorm output is never stored; its
-        // producer writes the pre-norm rows (xa: x + attention, xb: x1 + FFN) and every consumer applies the norm on
-        // the fly (GemmParams::a_ln_cs for GEMM inputs, res_ln_part for residual operands) from the partial row
-        // statistics the producer's epilogue leaves behind: enc_st_a belongs to xa (norm1), enc_st_b to xb (norm2).
-        for (int l = 0; l < kEncLayers; ++l) {
-            const EncLayer& e = m->enc[l];
-            const bool ln_in = l > 0;          // the layer input is LN2_{l-1}(xb), deferred
-            {
-                GemmParams p = gemm_base(T, 3 * kDModel, kDModel, cs(xin), kDModel, e.qkv.w, e.qkv.wtc, e.qkv.wtc_scale, w.qk, 2 * kDModel);
-                p.addmat = e.add_qkv_tc; p.add_period = kTokens; p.ld_add = 3 * kDModel;
-                p.remap = 1;
-                p.blk_map[0] = 0; p.blk_map[1] = kDModel; p.blk_map[2] = -1;
-                p.vt = w.vt; p.n_vt = 1;
-                p.kv_img = w.kvimg; p.blk_map[1] = -1000;           // keys and values go straight into the attention operand images
-                if (ln_in) { p.a_ln_cs = e.qkv.cs; p.a_ln_part = w.enc_st_b; }
-                if (launch_tc(r, p)) return 1;
-            }
-            AttnParams a{};
-            a.q = cs(w.qk); a.ldq = 2 * kDModel;
-            a.k = offset(cs(w.qk), kDModel); a.ldk = 2 * kDModel;
-            a.vt = cs(w.vt); a.vt_pair_stride = kVtLayer;
-            a.kv_img = w.kvimg; a.img_pair_stride = kHeads * kAttnHeadImgBytes;
-            a.out = w.ao; a.ldo = kDModel;
-            a.nq = kTokens; a.npairs = B; a.pair0 = 0;
-            if (run_attention(r, a)) return 1;
-            if (run_attention_weights(r, a, maps, l)) return 1;     // before the next layer overwrites qk / kvimg
-            // xa = x + out_proj(attn)                                   (transformer.py:149-154, norm1 deferred)
-            if (run_linear_dln(r, e.o, T, cs(w.ao), kDModel, w.xa, kDModel, false, nullptr, w.enc_st_a, cs(xin), kDModel,
-                               ln_in ? w.enc_st_b : nullptr, ln_in ? m->enc[l - 1].ln2_g : nullptr, ln_in ? m->enc[l - 1].ln2_b : nullptr)) return 1;
-            // h = relu(W1 norm1(xa) + b1)                               (transformer.py:155)
-            if (run_linear_dln(r, e.l1, T, cs(w.xa), kDModel, w.ffh, kFF, true, w.enc_st_a, nullptr)) return 1;
-            // xb = norm1(xa) + W2 h + b2                                (transformer.py:155-157, norm2 deferred)
-            if (run_linear_dln(r, e.l2, T, cs(w.ffh), kFF, w.xb, kDModel, false, nullptr, w.enc_st_b, cs(w.xa), kDModel,
-                               w.enc_st_a, e.ln1_g, e.ln1_b)) return 1;
-            xin = w.xb;
-        }
-        m->last_mem = xin;
-        m->last_mem_pre_ln = true;
-        // K / V projections of all 6 decoder layers from norm2(xb) of the last encoder layer (deferred as well)
-        {
-            GemmParams p = gemm_base(T, 2 * kKCols, kDModel, cs(xin), kDModel, m->kv_all.w, m->kv_all.wtc, m->kv_all.wtc_scale, ctx->k, kKCols);
-            p.addmat = m->add_kv_tc; p.add_period = kTokens; p.ld_add = 2 * kKCols;
-            p.remap = 1;
-            for (int l = 0; l < kDecLayers; ++l) {
-                p.blk_map[2 * l] = l * kDModel;
-                p.blk_map[2 * l + 1] = -(l + 1);
-            }
-            p.vt = ctx->vt; p.n_vt = kDecLayers;
-            p.kv_img = ctx->img;
-            for (int l = 0; l < kDecLayers; ++l) p.blk_map[2 * l] = -1000 - l;
-            p.a_ln_cs = m->kv_all.cs; p.a_ln_part = w.enc_st_b;
-            if (launch_tc(r, p)) return 1;
-        }
-        ctx->pairs = B;
-        ctx->holds_img = true;
-        m->last_pairs = B;
-        return 0;
-    }
-    // default schedule (and the fp32 SIMT cross-check path): explicit LayerNorm launches, the checkpoint's weights as they are
-    m->last_mem_pre_ln = false;
-    const bool tc = m->gemm_path == 0;      // tensor-core path: keys / values are written as attention operand images
+    // On the tensor-core path keys and values go straight into the attention operand images instead.
+    //
+    // Deferred LayerNorm (tensor-core path, see deferred_ln_enabled): no LayerNorm kernel and no LayerNorm epilogue.  A
+    // LayerNorm output is never stored; its producer writes the pre-norm rows (xa: x + attention, xb: x1 + FFN) and every
+    // consumer applies the norm on the fly (GemmParams::a_ln_cs for GEMM inputs, res_ln_part for residual operands) from
+    // the partial row statistics the producer's epilogue leaves behind: enc_st_a belongs to xa (norm1), enc_st_b to xb
+    // (norm2).  Otherwise (and on the fp32 SIMT cross-check path): explicit LayerNorm launches, the checkpoint's weights
+    // as they are.
+    const bool dln = deferred_ln_enabled(m, T);
+    const bool tc = m->gemm_path == 0;
     const bool fused_mlp = fused_mlp_enabled(m);
+    Split16 xin = w.src;      // layer input
     for (int l = 0; l < kEncLayers; ++l) {
         const EncLayer& e = m->enc[l];
+        const bool ln_in = dln && l > 0;          // the layer input is LN2_{l-1}(xb), deferred
         {
-            GemmParams p = gemm_base(T, 3 * kDModel, kDModel, cs(xin), kDModel, e.qkv.w, e.qkv.wtc_plain ? e.qkv.wtc_plain : e.qkv.wtc, e.qkv.wtc_plain ? e.qkv.wtc_plain_scale : e.qkv.wtc_scale, w.qk, 2 * kDModel);
-            p.addmat = e.add_qkv; p.add_period = kTokens; p.ld_add = 3 * kDModel;
-            p.remap = 1;
-            p.blk_map[0] = 0; p.blk_map[1] = kDModel; p.blk_map[2] = -1;
-            p.vt = w.vt; p.n_vt = 1;
-            if (tc) { p.kv_img = w.kvimg; p.blk_map[1] = -1000; }
+            GemmParams p = gemm_linear(e.qkv, dln, T, cs(xin), kDModel, w.qk, 2 * kDModel);
+            p.addmat = dln ? e.add_qkv_tc : e.add_qkv; p.add_period = kTokens; p.ld_add = 3 * kDModel;
+            redirect_kv(p, 1, 1, kDModel, w.vt, tc ? w.kvimg : nullptr);
+            if (ln_in) { p.a_ln_cs = e.qkv.cs; p.a_ln_part = w.enc_st_b; }
             if (run_gemm(r, p, nullptr)) return 1;
         }
         AttnParams a{};
@@ -800,34 +865,39 @@ int encode_tail(cotr_model* m, CSplit16 feat, const int* pairs, int B, cotr_cont
         a.nq = kTokens; a.npairs = B; a.pair0 = 0;
         if (run_attention(r, a)) return 1;
         if (run_attention_weights(r, a, maps, l)) return 1;         // before the next layer overwrites qk / kvimg
-        // x1 = LN1(x + out_proj(attn))
-        if (run_linear(r, e.o, T, cs(w.ao), kDModel, w.xa, kDModel, false, cs(xin), kDModel, e.ln1_g, e.ln1_b, w.ln_tmp)) return 1;
-        // x2 = LN2(x1 + W2 relu(W1 x1 + b1) + b2)
-        if (fused_mlp) {
-            if (run_mlp(r, e.l1, e.l2, T, cs(w.xa), w.xb, e.ln2_g, e.ln2_b)) return 1;
+        if (dln) {
+            // xa = x + out_proj(attn)                                   (transformer.py:149-154, norm1 deferred)
+            if (run_linear_dln(r, e.o, T, cs(w.ao), kDModel, w.xa, kDModel, false, nullptr, w.enc_st_a, cs(xin), kDModel,
+                               ln_in ? w.enc_st_b : nullptr, ln_in ? m->enc[l - 1].ln2_g : nullptr, ln_in ? m->enc[l - 1].ln2_b : nullptr)) return 1;
+            // h = relu(W1 norm1(xa) + b1)                               (transformer.py:155)
+            if (run_linear_dln(r, e.l1, T, cs(w.xa), kDModel, w.ffh, kFF, true, w.enc_st_a, nullptr)) return 1;
+            // xb = norm1(xa) + W2 h + b2                                (transformer.py:155-157, norm2 deferred)
+            if (run_linear_dln(r, e.l2, T, cs(w.ffh), kFF, w.xb, kDModel, false, nullptr, w.enc_st_b, cs(w.xa), kDModel,
+                               w.enc_st_a, e.ln1_g, e.ln1_b)) return 1;
         } else {
-            if (run_linear(r, e.l1, T, cs(w.xa), kDModel, w.ffh, kFF, true)) return 1;
-            if (run_linear(r, e.l2, T, cs(w.ffh), kFF, w.xb, kDModel, false, cs(w.xa), kDModel, e.ln2_g, e.ln2_b, w.ln_tmp)) return 1;
+            // x1 = LN1(x + out_proj(attn))
+            if (run_linear(r, e.o, T, cs(w.ao), kDModel, w.xa, kDModel, false, cs(xin), kDModel, e.ln1_g, e.ln1_b, w.ln_tmp)) return 1;
+            // x2 = LN2(x1 + W2 relu(W1 x1 + b1) + b2)
+            if (fused_mlp) {
+                if (run_mlp(r, e.l1, e.l2, T, cs(w.xa), w.xb, e.ln2_g, e.ln2_b)) return 1;
+            } else {
+                if (run_linear(r, e.l1, T, cs(w.xa), kDModel, w.ffh, kFF, true)) return 1;
+                if (run_linear(r, e.l2, T, cs(w.ffh), kFF, w.xb, kDModel, false, cs(w.xa), kDModel, e.ln2_g, e.ln2_b, w.ln_tmp)) return 1;
+            }
         }
         xin = w.xb;
     }
     m->last_mem = xin;
+    m->last_mem_pre_ln = dln;
 
     // transformer.py:192-195: K_l = (mem + pos) Wk_l^T + bk_l, V_l = mem Wv_l^T + bv_l for all 6 decoder layers in ONE
-    // GEMM (N = 3072): K blocks go row-major into ctx->k [T][1536], V blocks transposed into ctx->vt [pair][6][256][512].
+    // GEMM (N = 3072): K blocks go row-major into ctx->k [T][1536], V blocks transposed into ctx->vt [pair][6][256][512]
+    // (or both into the context's operand images).  Deferred: mem is norm2(xb) of the last encoder layer, applied here.
     {
-        GemmParams p = gemm_base(T, 2 * kKCols, kDModel, cs(xin), kDModel, m->kv_all.w, m->kv_all.wtc_plain ? m->kv_all.wtc_plain : m->kv_all.wtc, m->kv_all.wtc_plain ? m->kv_all.wtc_plain_scale : m->kv_all.wtc_scale, ctx->k, kKCols);
-        p.addmat = m->add_kv; p.add_period = kTokens; p.ld_add = 2 * kKCols;
-        p.remap = 1;
-        for (int l = 0; l < kDecLayers; ++l) {
-            p.blk_map[2 * l] = l * kDModel;
-            p.blk_map[2 * l + 1] = -(l + 1);
-        }
-        p.vt = ctx->vt; p.n_vt = kDecLayers;
-        if (tc) {
-            p.kv_img = ctx->img;
-            for (int l = 0; l < kDecLayers; ++l) p.blk_map[2 * l] = -1000 - l;
-        }
+        GemmParams p = gemm_linear(m->kv_all, dln, T, cs(xin), kDModel, ctx->k, kKCols);
+        p.addmat = dln ? m->add_kv_tc : m->add_kv; p.add_period = kTokens; p.ld_add = 2 * kKCols;
+        redirect_kv(p, 0, kDecLayers, 0, ctx->vt, tc ? ctx->img : nullptr);
+        if (dln) { p.a_ln_cs = m->kv_all.cs; p.a_ln_part = w.enc_st_b; }
         if (run_gemm(r, p, nullptr)) return 1;
     }
     ctx->pairs = B;
@@ -840,6 +910,15 @@ int check_context(cotr_model* m, const char* fn, int B, const cotr_context* ctx)
     COTR_CHECK(B >= 1, "%s: B must be >= 1 (got %d)", fn, B);
     COTR_CHECK(ctx && ctx->model == m, "%s: context does not belong to this model", fn);
     COTR_CHECK(B <= ctx->max_pairs, "%s: B = %d exceeds the context capacity %d", fn, B, ctx->max_pairs);
+    return 0;
+}
+
+// A decode's context: this model's, holding exactly B pairs, encoded under the current matrix-multiply path.
+int check_decode_context(cotr_model* m, const char* fn, int B, const cotr_context* ctx) {
+    COTR_CHECK(ctx && ctx->model == m, "%s: context does not belong to this model", fn);
+    COTR_CHECK(B >= 1 && B == ctx->pairs, "%s: B = %d but the context holds %d pairs", fn, B, ctx->pairs);
+    COTR_CHECK(ctx->holds_img == (m->gemm_path == 0), "%s: the context was encoded under the other matrix-multiply path "
+               "(cotr_set_gemm_path): re-encode it", fn);
     return 0;
 }
 
@@ -872,23 +951,9 @@ int encode_images_impl(cotr_model* m, const float* img, int N, void* feat_dev, c
 int encode_pairs_impl(cotr_model* m, const void* feat_dev, int n_images, const int32_t* pairs, int B, cotr_context* ctx,
                       cudaStream_t s, const AttnMaps& maps) {
     if (ensure_encode_ws(m, B)) return 1;
-    if (B > m->pair_cap) {
-        COTR_CHECK_CUDA(cudaDeviceSynchronize());
-        if (m->pair_tab) { cudaFree(m->pair_tab); m->pair_tab = nullptr; }
-        if (m->pair_stage) { cudaFreeHost(m->pair_stage); m->pair_stage = nullptr; }
-        m->pair_cap = 0;
-        COTR_CHECK_CUDA(cudaMalloc((void**)&m->pair_tab, 2 * (size_t)B * sizeof(int)));
-        COTR_CHECK_CUDA(cudaMallocHost((void**)&m->pair_stage, 2 * (size_t)B * sizeof(int)));
-        m->pair_cap = B;
-    }
-    if (!m->pair_copied) COTR_CHECK_CUDA(cudaEventCreateWithFlags(&m->pair_copied, cudaEventDisableTiming));
-    // the previous call's copy out of the staging buffer has long completed unless the host runs a whole call ahead
-    COTR_CHECK_CUDA(cudaEventSynchronize(m->pair_copied));
-    memcpy(m->pair_stage, pairs, 2 * (size_t)B * sizeof(int));
-    COTR_CHECK_CUDA(cudaMemcpyAsync(m->pair_tab, m->pair_stage, 2 * (size_t)B * sizeof(int), cudaMemcpyHostToDevice, s));
-    COTR_CHECK_CUDA(cudaEventRecord(m->pair_copied, s));
+    if (m->pair_tab.upload(pairs, 2 * (size_t)B, s)) return 1;
     const __half* hi = static_cast<const __half*>(feat_dev);
-    return encode_tail(m, CSplit16{hi, hi + (size_t)n_images * kFeatElems}, m->pair_tab, B, ctx, s, maps);
+    return encode_tail(m, CSplit16{hi, hi + (size_t)n_images * kFeatElems}, m->pair_tab.dev, B, ctx, s, maps);
 }
 
 // R query rows (queries / pred: (R,2)).  tiles == nullptr: pair pair0 + p owns rows p * nq .. p * nq + nq - 1, p < npairs;
@@ -899,7 +964,6 @@ int decode_chunk(cotr_model* m, const cotr_context* ctx, const float* queries, f
     Workspace& w = m->ws;
     Run r{m, s};
     const CSplit16 none{nullptr, nullptr};
-    auto attend = [&](const AttnParams& a) { return tiles ? run_attention_tiles(r, a, *tiles) : run_attention(r, a); };
     // cotr_model.py:34-35 query_proj (lin_sine, depth 64)
     {
         LaunchScope scope(r, K_QENC, R, kDModel, 0);
@@ -909,63 +973,43 @@ int decode_chunk(cotr_model* m, const cotr_context* ctx, const float* queries, f
     // all 6 layers is one GEMM.
     if (run_linear(r, m->qpos_all, R, cs(w.qpos), kDModel, w.qp, kQpCols, false)) return 1;
 
-    if (deferred_ln_enabled(m, R)) {
-        // Tensor-core path with deferred LayerNorms (see encode_impl): w.t = t + attention (norm2 deferred),
-        // w.t2 = t1 + FFN (norm3 deferred); dec_st_a = partial row statistics of w.t (norm2), dec_st_b of w.t2 (norm3).
-        for (int l = 0; l < kDecLayers; ++l) {
-            const DecLayer& d = m->dec[l];
-            const bool ln_in = l > 0;
-            CSplit16 q = cs(w.qp);      // layer 0: tgt = 0 (transformer.py:54), so q is the qpos projection alone
-            int ldq = kQpCols;
-            if (ln_in) {
-                if (run_linear_dln(r, d.q, R, cs(w.t2), kDModel, w.qb, kDModel, false, w.dec_st_b, nullptr,
-                                   offset(cs(w.qp), (size_t)l * kDModel), kQpCols)) return 1;
-                q = cs(w.qb); ldq = kDModel;
-            }
-            AttnParams a{};
-            a.q = q; a.ldq = ldq;
-            a.k = offset(cs(ctx->k), (size_t)l * kDModel); a.ldk = kKCols;
-            a.vt = offset(cs(ctx->vt), (size_t)l * kVtLayer); a.vt_pair_stride = kDecLayers * kVtLayer;
-            if (ctx->holds_img) { a.kv_img = ctx->img + (size_t)l * kHeads * kAttnHeadImgBytes; a.img_pair_stride = (size_t)kDecLayers * kHeads * kAttnHeadImgBytes; }
-            a.out = w.dao; a.ldo = kDModel;
-            a.nq = nq; a.npairs = npairs; a.pair0 = pair0;
-            if (attend(a)) return 1;
-            if (run_attention_weights(r, a, maps, l)) return 1;
+    // Deferred LayerNorm (see encode_tail): w.t = t + attention (norm2 deferred), w.t2 = t1 + FFN (norm3 deferred);
+    // dec_st_a = partial row statistics of w.t (norm2), dec_st_b of w.t2 (norm3).  Explicit: every layer ends in w.t.
+    const bool dln = deferred_ln_enabled(m, R);
+    const bool fused_mlp = fused_mlp_enabled(m);
+    const Split16 tin = dln ? w.t2 : w.t;      // the layer input t of layers > 0 (deferred: before norm3_{l-1})
+    for (int l = 0; l < kDecLayers; ++l) {
+        const DecLayer& d = m->dec[l];
+        const bool ln_in = dln && l > 0;
+        CSplit16 q = cs(w.qp);      // layer 0: tgt = 0 (transformer.py:54), so q is the qpos projection alone
+        int ldq = kQpCols;
+        if (l > 0) {
+            const CSplit16 qpos_l = offset(cs(w.qp), (size_t)l * kDModel);
+            if (dln ? run_linear_dln(r, d.q, R, cs(tin), kDModel, w.qb, kDModel, false, w.dec_st_b, nullptr, qpos_l, kQpCols)
+                    : run_linear(r, d.q, R, cs(tin), kDModel, w.qb, kDModel, false, qpos_l, kQpCols)) return 1;
+            q = cs(w.qb); ldq = kDModel;
+        }
+        AttnParams a{};
+        a.q = q; a.ldq = ldq;
+        a.k = offset(cs(ctx->k), (size_t)l * kDModel); a.ldk = kKCols;
+        a.vt = offset(cs(ctx->vt), (size_t)l * kVtLayer); a.vt_pair_stride = kDecLayers * kVtLayer;
+        if (ctx->holds_img) { a.kv_img = ctx->img + (size_t)l * kHeads * kAttnHeadImgBytes; a.img_pair_stride = (size_t)kDecLayers * kHeads * kAttnHeadImgBytes; }
+        a.out = w.dao; a.ldo = kDModel;
+        a.nq = nq; a.npairs = npairs; a.pair0 = pair0;
+        if (run_attention(r, a, tiles)) return 1;
+        if (run_attention_weights(r, a, maps, l)) return 1;
+        const CSplit16 res = l > 0 ? cs(tin) : none;
+        if (dln) {
             // transformer.py:196-197: t = t + out_proj(attn)   (norm2 deferred; t = norm3_{l-1}(t2), deferred, or 0)
-            if (run_linear_dln(r, d.o, R, cs(w.dao), kDModel, w.t, kDModel, false, nullptr, w.dec_st_a, ln_in ? cs(w.t2) : none, kDModel,
+            if (run_linear_dln(r, d.o, R, cs(w.dao), kDModel, w.t, kDModel, false, nullptr, w.dec_st_a, res, kDModel,
                                ln_in ? w.dec_st_b : nullptr, ln_in ? m->dec[l - 1].ln3_g : nullptr, ln_in ? m->dec[l - 1].ln3_b : nullptr)) return 1;
             // transformer.py:198-200: t2 = norm2(t) + linear2(relu(linear1(norm2(t))))   (norm3 deferred)
             if (run_linear_dln(r, d.l1, R, cs(w.t), kDModel, w.dh, kFF, true, w.dec_st_a, nullptr)) return 1;
             if (run_linear_dln(r, d.l2, R, cs(w.dh), kFF, w.t2, kDModel, false, nullptr, w.dec_st_b, cs(w.t), kDModel,
                                w.dec_st_a, d.ln2_g, d.ln2_b)) return 1;
-        }
-        // norm3 of the last layer, then transformer.py:110-111 decoder.norm, in one pass over the rows
-        {
-            const DecLayer& d = m->dec[kDecLayers - 1];
-            LaunchScope scope(r, K_LAYERNORM, R, kDModel, 0);
-            if (launch_layernorm_twice(cs(w.t2), d.ln3_g, d.ln3_b, m->dec_norm_g, m->dec_norm_b, w.hs, R, s)) return 1;
-        }
-    } else {
-        const bool fused_mlp = fused_mlp_enabled(m);
-        for (int l = 0; l < kDecLayers; ++l) {
-            const DecLayer& d = m->dec[l];
-            CSplit16 q = cs(w.qp);      // layer 0: tgt = 0 (transformer.py:54), so q is the qpos projection alone
-            int ldq = kQpCols;
-            if (l > 0) {
-                if (run_linear(r, d.q, R, cs(w.t), kDModel, w.qb, kDModel, false, offset(cs(w.qp), (size_t)l * kDModel), kQpCols)) return 1;
-                q = cs(w.qb); ldq = kDModel;
-            }
-            AttnParams a{};
-            a.q = q; a.ldq = ldq;
-            a.k = offset(cs(ctx->k), (size_t)l * kDModel); a.ldk = kKCols;
-            a.vt = offset(cs(ctx->vt), (size_t)l * kVtLayer); a.vt_pair_stride = kDecLayers * kVtLayer;
-            if (ctx->holds_img) { a.kv_img = ctx->img + (size_t)l * kHeads * kAttnHeadImgBytes; a.img_pair_stride = (size_t)kDecLayers * kHeads * kAttnHeadImgBytes; }
-            a.out = w.dao; a.ldo = kDModel;
-            a.nq = nq; a.npairs = npairs; a.pair0 = pair0;
-            if (attend(a)) return 1;
-            if (run_attention_weights(r, a, maps, l)) return 1;
+        } else {
             // transformer.py:196-197: t = norm2(t + out_proj(attn))
-            if (run_linear(r, d.o, R, cs(w.dao), kDModel, w.t, kDModel, false, l > 0 ? cs(w.t) : none, kDModel, d.ln2_g, d.ln2_b, w.dln_tmp)) return 1;
+            if (run_linear(r, d.o, R, cs(w.dao), kDModel, w.t, kDModel, false, res, kDModel, d.ln2_g, d.ln2_b, w.dln_tmp)) return 1;
             // transformer.py:198-200: t = norm3(t + linear2(relu(linear1(t))))
             if (fused_mlp) {
                 // in place; the last layer also applies transformer.py:110-111 decoder.norm and writes hs
@@ -977,11 +1021,16 @@ int decode_chunk(cotr_model* m, const cotr_context* ctx, const float* queries, f
                 if (run_linear(r, d.l2, R, cs(w.dh), kFF, w.t, kDModel, false, cs(w.t), kDModel, d.ln3_g, d.ln3_b, w.dln_tmp)) return 1;
             }
         }
-        // transformer.py:110-111 decoder.norm on the last level; cotr_model.py:38-39 corr_embed on that level only.
-        if (!fused_mlp) {
-            LaunchScope scope(r, K_LAYERNORM, R, kDModel, 0);
-            if (launch_layernorm(cs(w.t), m->dec_norm_g, m->dec_norm_b, w.hs, R, s)) return 1;
-        }
+    }
+    // transformer.py:110-111 decoder.norm on the last level; cotr_model.py:38-39 corr_embed on that level only.
+    if (dln) {
+        // norm3 of the last layer, then decoder.norm, in one pass over the rows
+        const DecLayer& d = m->dec[kDecLayers - 1];
+        LaunchScope scope(r, K_LAYERNORM, R, kDModel, 0);
+        if (launch_layernorm_twice(cs(w.t2), d.ln3_g, d.ln3_b, m->dec_norm_g, m->dec_norm_b, w.hs, R, s)) return 1;
+    } else if (!fused_mlp) {      // (fused: the last feed-forward launch wrote hs)
+        LaunchScope scope(r, K_LAYERNORM, R, kDModel, 0);
+        if (launch_layernorm(cs(w.t), m->dec_norm_g, m->dec_norm_b, w.hs, R, s)) return 1;
     }
     if (run_linear(r, m->head[0], R, cs(w.hs), kDModel, w.hd1, kDModel, true)) return 1;
     if (run_linear(r, m->head[1], R, cs(w.hd1), kDModel, w.hd2, kDModel, true)) return 1;
@@ -997,11 +1046,8 @@ int decode_chunk(cotr_model* m, const cotr_context* ctx, const float* queries, f
 // maps (optional): base = attn_dev, layer_stride = B * Q * 512, pair_stride = Q * 512
 int decode_impl(cotr_model* m, const cotr_context* ctx, const float* queries, int B, int Q, float* pred, cudaStream_t s,
                 const AttnMaps& maps = AttnMaps()) {
-    COTR_CHECK(ctx && ctx->model == m, "cotr_decode: context does not belong to this model");
-    COTR_CHECK(B >= 1 && B == ctx->pairs, "cotr_decode: B = %d but the context holds %d pairs", B, ctx ? ctx->pairs : -1);
+    if (check_decode_context(m, "cotr_decode", B, ctx)) return 1;
     COTR_CHECK(Q >= 0, "cotr_decode: negative Q");
-    COTR_CHECK(ctx->holds_img == (m->gemm_path == 0), "cotr_decode: the context was encoded under the other matrix-multiply path "
-               "(cotr_set_gemm_path): re-encode it");
     if (Q == 0) return 0;
     COTR_CHECK_CUDA(cudaSetDevice(m->device));
     const long long total = (long long)B * Q;
@@ -1089,24 +1135,9 @@ int decode_ragged_impl(cotr_model* m, const cotr_context* ctx, const float* quer
     int cap = 0;
     for (const Chunk& c : chunks) cap = std::max(cap, c.rows);
     if (ensure_decode_ws(m, cap)) return 1;
-    if (tab.size() > m->tile_cap) {
-        COTR_CHECK_CUDA(cudaDeviceSynchronize());
-        m->tile_cap = 0;      // as in ensure_decode_ws: no stale capacity after a failed allocation
-        if (m->tile_tab) { cudaFree(m->tile_tab); m->tile_tab = nullptr; }
-        if (m->tile_stage) { cudaFreeHost(m->tile_stage); m->tile_stage = nullptr; }
-        COTR_CHECK_CUDA(cudaMalloc((void**)&m->tile_tab, tab.size() * sizeof(int4)));
-        COTR_CHECK_CUDA(cudaMallocHost((void**)&m->tile_stage, tab.size() * sizeof(int4)));
-        m->tile_cap = tab.size();
-    }
-    if (!m->tile_copied) COTR_CHECK_CUDA(cudaEventCreateWithFlags(&m->tile_copied, cudaEventDisableTiming));
-    // as in encode_pairs_impl: the previous call's copy out of the staging buffer has long completed unless the host
-    // runs a whole call ahead of the device
-    COTR_CHECK_CUDA(cudaEventSynchronize(m->tile_copied));
-    memcpy(m->tile_stage, tab.data(), tab.size() * sizeof(int4));
-    COTR_CHECK_CUDA(cudaMemcpyAsync(m->tile_tab, m->tile_stage, tab.size() * sizeof(int4), cudaMemcpyHostToDevice, s));
-    COTR_CHECK_CUDA(cudaEventRecord(m->tile_copied, s));
+    if (m->tile_tab.upload(tab.data(), tab.size(), s)) return 1;
     for (Chunk& c : chunks) {
-        c.t.tab = m->tile_tab + c.tab0;
+        c.t.tab = m->tile_tab.dev + c.tab0;
         const size_t off = (size_t)c.row0 * 2;
         if (decode_chunk(m, ctx, queries + off, pred + off, c.rows, &c.t, 0, 0, 0, s, AttnMaps())) return 1;
     }
@@ -1261,24 +1292,20 @@ int build_model(cotr_model* m, const TensorMap& tm) {
     if (linear_from("corr_embed.layers.2", 2, kDModel, &m->head[2])) return 1;
 
     // add matrices: pos [512,256] x Wmasked^T + bias  (fp32 SIMT GEMM on the split16 pos table, fp32 result)
-    Split16 pos16 = kNoSplit;
-    if (ws_alloc(&pos16, (size_t)kTokens * kDModel)) return 1;
-    if (launch_f32_to_split16(m->pos, pos16, (size_t)kTokens * kDModel, 0)) return 1;
+    TmpSplit pos16;
+    if (pos16.from_f32(m->pos, (size_t)kTokens * kDModel)) return 1;
     for (PosBiasJob& j : jobs) {
+        DevAllocs tmp;
         float *wd = nullptr, *bd = nullptr;
-        COTR_CHECK_CUDA(cudaMalloc((void**)&wd, j.w_masked.size() * sizeof(float)));
-        COTR_CHECK_CUDA(cudaMalloc((void**)&bd, j.bias.size() * sizeof(float)));
-        COTR_CHECK_CUDA(cudaMemcpy(wd, j.w_masked.data(), j.w_masked.size() * sizeof(float), cudaMemcpyHostToDevice));
-        COTR_CHECK_CUDA(cudaMemcpy(bd, j.bias.data(), j.bias.size() * sizeof(float), cudaMemcpyHostToDevice));
+        if (tmp.upload((void**)&wd, j.w_masked.data(), j.w_masked.size() * sizeof(float)) ||
+            tmp.upload((void**)&bd, j.bias.data(), j.bias.size() * sizeof(float)))
+            return 1;
         if (dev_alloc(m, (void**)j.dst, (size_t)kTokens * j.N * sizeof(float))) return 1;
-        GemmParams p = gemm_base(kTokens, j.N, kDModel, cs(pos16), kDModel, wd, nullptr, 1.f, kNoSplit, j.N);
+        GemmParams p = gemm_base(kTokens, j.N, kDModel, cs(pos16.t), kDModel, wd, nullptr, 1.f, kNoSplit, j.N);
         p.bias = bd;
         if (launch_gemm_simt_raw(p, *j.dst, 0)) return 1;
         COTR_CHECK_CUDA(cudaDeviceSynchronize());
-        cudaFree(wd);
-        cudaFree(bd);
     }
-    ws_free(&pos16);
     if (!m->enc[0].add_qkv_tc) m->enc[0].add_qkv_tc = m->enc[0].add_qkv;     // layer 0 reads the un-normalised input projection
     return 0;
 }
@@ -1331,21 +1358,9 @@ void cotr_destroy(cotr_model* m) {
     if (m->own_ctx) cotr_context_destroy(m->own_ctx);
     for (void* p : m->allocs) cudaFree(p);
     Workspace& w = m->ws;
-    Split16* bufs[] = {&w.canvas, &w.stem, &w.bx, &w.by, &w.bt1, &w.bt2, &w.bds, &w.src, &w.xa, &w.xb, &w.qk, &w.vt, &w.ao, &w.ffh,
-                       &w.qpos, &w.qp, &w.t, &w.qb, &w.dao, &w.dh, &w.hs, &w.hd1, &w.hd2, &w.t2};
-    for (Split16* b : bufs) ws_free(b);
-    if (w.kvimg) cudaFree(w.kvimg);
-    if (w.pair_id) cudaFree(w.pair_id);
-    if (m->pair_tab) cudaFree(m->pair_tab);
-    if (m->pair_stage) cudaFreeHost(m->pair_stage);
-    if (m->pair_copied) cudaEventDestroy(m->pair_copied);
-    if (m->tile_tab) cudaFree(m->tile_tab);
-    if (m->tile_stage) cudaFreeHost(m->tile_stage);
-    if (m->tile_copied) cudaEventDestroy(m->tile_copied);
-    float** fbufs[] = {&w.ln_tmp, &w.dln_tmp, &w.img_stage, &w.q_stage, &w.pred_stage,
-                       reinterpret_cast<float**>(&w.enc_st_a), reinterpret_cast<float**>(&w.enc_st_b),
-                       reinterpret_cast<float**>(&w.dec_st_a), reinterpret_cast<float**>(&w.dec_st_b)};
-    for (float** b : fbufs) ws_free_f32(b);
+    ws_release(encode_ws_bufs(w, 0));
+    ws_release(decode_ws_bufs(w, 0));
+    for (float** b : {&w.img_stage, &w.q_stage, &w.pred_stage}) ws_free_f32(b);
     if (m->host_stream) cudaStreamDestroy(m->host_stream);
     for (auto& kv : m->graphs) cudaGraphExecDestroy(kv.second);
     preprocessor_destroy(m->pre);
@@ -1401,10 +1416,7 @@ int cotr_decode_ragged(cotr_model* m, const cotr_context* ctx, const float* quer
     const char* fn = "cotr_decode_ragged";
     COTR_CHECK(m != nullptr, "%s: null model", fn);
     m->launches = 0;
-    COTR_CHECK(ctx && ctx->model == m, "%s: context does not belong to this model", fn);
-    COTR_CHECK(B >= 1 && B == ctx->pairs, "%s: B = %d but the context holds %d pairs", fn, B, ctx->pairs);
-    COTR_CHECK(ctx->holds_img == (m->gemm_path == 0), "%s: the context was encoded under the other matrix-multiply path "
-               "(cotr_set_gemm_path): re-encode it", fn);
+    if (check_decode_context(m, fn, B, ctx)) return 1;
     COTR_CHECK(offsets_host != nullptr, "%s: null offsets_host", fn);
     COTR_CHECK(offsets_host[0] == 0, "%s: offsets_host[0] = %lld, must be 0", fn, (long long)offsets_host[0]);
     for (int p = 0; p < B; ++p)
@@ -1434,12 +1446,7 @@ int cotr_encode_context_attention(cotr_model* m, const float* img_dev, int B, co
     COTR_CHECK_CUDA(cudaSetDevice(m->device));
     CallOrder order(m, (cudaStream_t)cuda_stream);
     m->launches = 0;
-    AttnMaps maps;
-    maps.mask = (unsigned)layer_mask;
-    maps.base = attn_dev;
-    maps.layer_stride = (size_t)B * kTokens * kTokens;
-    maps.pair_stride = (size_t)kTokens * kTokens;
-    return encode_impl(m, img_dev, B, ctx, (cudaStream_t)cuda_stream, maps);
+    return encode_impl(m, img_dev, B, ctx, (cudaStream_t)cuda_stream, attn_maps(layer_mask, attn_dev, B, kTokens));
 }
 
 int cotr_encode_images(cotr_model* m, const float* img_dev, int N, void* feat_dev, void* cuda_stream) {
@@ -1468,12 +1475,8 @@ int cotr_encode_context_pairs(cotr_model* m, const void* feat_dev, int n_images,
     COTR_CHECK_CUDA(cudaSetDevice(m->device));
     CallOrder order(m, (cudaStream_t)cuda_stream);
     m->launches = 0;
-    AttnMaps maps;
-    maps.mask = (unsigned)layer_mask;
-    maps.base = attn_dev;
-    maps.layer_stride = (size_t)B * kTokens * kTokens;
-    maps.pair_stride = (size_t)kTokens * kTokens;
-    return encode_pairs_impl(m, feat_dev, n_images, pairs_host, B, ctx, (cudaStream_t)cuda_stream, maps);
+    return encode_pairs_impl(m, feat_dev, n_images, pairs_host, B, ctx, (cudaStream_t)cuda_stream,
+                             attn_maps(layer_mask, attn_dev, B, kTokens));
 }
 
 int cotr_decode_attention(cotr_model* m, const cotr_context* ctx, const float* queries_dev, int B, int Q, int layer_mask,
@@ -1483,12 +1486,7 @@ int cotr_decode_attention(cotr_model* m, const cotr_context* ctx, const float* q
     COTR_CHECK_CUDA(cudaSetDevice(m->device));
     CallOrder order(m, (cudaStream_t)cuda_stream);
     m->launches = 0;
-    AttnMaps maps;
-    maps.mask = (unsigned)layer_mask;
-    maps.base = attn_dev;
-    maps.layer_stride = (size_t)B * Q * kTokens;
-    maps.pair_stride = (size_t)Q * kTokens;
-    return decode_impl(m, ctx, queries_dev, B, Q, pred_dev, (cudaStream_t)cuda_stream, maps);
+    return decode_impl(m, ctx, queries_dev, B, Q, pred_dev, (cudaStream_t)cuda_stream, attn_maps(layer_mask, attn_dev, B, Q));
 }
 
 namespace {
@@ -1656,7 +1654,8 @@ size_t cotr_workspace_bytes(int B, int Q) {
     if (B < 1 || Q < 0) return 0;
     const long long total = (long long)B * Q;
     const int rows = (int)(total < kDecodeChunkRows ? total : kDecodeChunkRows);
-    return (encode_ws_elems(B) + decode_ws_elems(rows)) * sizeof(float);
+    Workspace w;
+    return ws_bytes(encode_ws_bufs(w, B)) + ws_bytes(decode_ws_bufs(w, rows));
 }
 
 int cotr_last_launch_count(const cotr_model* m) { return m ? m->launches : -1; }
@@ -1686,13 +1685,6 @@ int cotr_profile_end(cotr_model* m, cotr_launch_record* out, int max_records) {
     return -n - 1;     // see header: success is encoded as -(count + 1)
 }
 
-namespace {
-struct TmpSplitDbg {
-    Split16 t = kNoSplit;
-    ~TmpSplitDbg() { ws_free(&t); }
-};
-}  // namespace
-
 int64_t cotr_debug_read(cotr_model* m, const char* name, float* out_host, int64_t max_elems) {
     if (!m || !name || !out_host) return -1;
     cudaSetDevice(m->device);
@@ -1704,7 +1696,7 @@ int64_t cotr_debug_read(cotr_model* m, const char* name, float* out_host, int64_
     if (s == "feat") { src = cs(m->last_feat); n = (int64_t)m->last_pairs * 2 * 16 * 16 * 1024; }
     else if (s == "src") { src = cs(m->ws.src); n = (int64_t)m->last_pairs * kTokens * kDModel; }
     else if (s == "mem") { src = cs(m->last_mem); n = (int64_t)m->last_pairs * kTokens * kDModel; }
-    TmpSplitDbg mem_ln;
+    TmpSplit mem_ln;
     if (s == "mem" && m->last_mem_pre_ln && src.hi && n > 0) {
         // tensor-core path: the encoder output exists only before its last (deferred) LayerNorm - apply it here
         const EncLayer& e = m->enc[kEncLayers - 1];
@@ -1754,16 +1746,33 @@ void cotr_debug_set_variant(int variant) { g_tc_variant = variant; g_use_pdl = (
 
 // ---- kernel-level test hooks: fp32 device tensors in / out, converted to split16 around the kernel under test -------
 namespace {
-struct TmpSplit {
-    Split16 t = kNoSplit;
-    ~TmpSplit() { ws_free(&t); }
-    int from_f32(const float* src, size_t n) {
-        const size_t padded = (n + 7) & ~(size_t)7;
-        if (ws_alloc(&t, padded)) return 1;
-        return launch_f32_to_split16(src, t, n, 0);
-    }
-    int empty(size_t n) { return ws_alloc(&t, (n + 7) & ~(size_t)7); }
-};
+// tensor-core image of a host [N,K] weight, as the model uploads it; returns acc_scale in *scale
+int upload_tc_weight(DevAllocs& mem, const float* w_host, int N, int K, void** wtc, float* scale) {
+    std::vector<uint8_t> img(tc_weight_bytes(N, K));
+    *scale = tc_pack_weight(w_host, N, K, img.data());
+    return mem.upload(wtc, img.data(), img.size());
+}
+
+std::vector<float> identity(int n) {
+    std::vector<float> eye((size_t)n * n, 0.f);
+    for (int i = 0; i < n; ++i) eye[(size_t)i * n + i] = 1.f;
+    return eye;
+}
+
+// Writes the keys (kv: [rows][256]) or the keys and values (kv: [rows][512] = [K | V]) of every pair into slot `slot`
+// of the `slots` attention operand images per pair at img, by the same epilogue store as the model's projections: a
+// tensor-core GEMM with the identity as its weight.
+int write_operand_images(DevAllocs& mem, CSplit16 kv, int rows, bool values, int slot, int slots, unsigned char* img) {
+    const int n = values ? 2 * kDModel : kDModel;
+    const std::vector<float> eye = identity(n);
+    void* wtc = nullptr;
+    float scale = 1.f;
+    if (upload_tc_weight(mem, eye.data(), n, n, &wtc, &scale)) return 1;
+    GemmParams p = gemm_base(rows, n, n, kv, n, nullptr, wtc, scale, kNoSplit, n);
+    p.remap = 1; p.blk_map[0] = -1000 - slot; p.n_vt = slots; p.kv_img = img;
+    if (values) p.blk_map[1] = -(slot + 1);
+    return launch_gemm_tc(p, 0);
+}
 }  // namespace
 
 int cotr_test_gemm(const cotr_test_gemm_desc* d, const float* A_dev, const float* w_host, const float* bias_dev,
@@ -1783,6 +1792,7 @@ int cotr_test_gemm(const cotr_test_gemm_desc* d, const float* A_dev, const float
     COTR_CHECK(!dln || (d->path == 0 && ln_gamma_dev && ln_beta_dev), "cotr_test_gemm: deferred LayerNorm needs path 0 and gamma / beta");
     if (!dln) { p.ln_gamma = ln_gamma_dev; p.ln_beta = ln_beta_dev; }
     p.ldc = d->ldc;
+    DevAllocs mem;
     TmpSplit a16, res16, out16;
     int K = d->K;
     std::vector<float> w_stem;
@@ -1803,12 +1813,11 @@ int cotr_test_gemm(const cotr_test_gemm_desc* d, const float* A_dev, const float
         if (a16.from_f32(A_dev, (size_t)d->a_elems)) return 1;
         p.a = cs(a16.t);
     }
-    int* pair_id = nullptr;
     if (d->a_mode == A_TOKENS) {            // the canvas order, as cotr_encode_context runs it: pair p = images (2p, 2p+1)
         std::vector<int> ident(2 * (size_t)((d->M + kTokens - 1) / kTokens));
         for (size_t i = 0; i < ident.size(); ++i) ident[i] = (int)i;
-        COTR_CHECK_CUDA(cudaMalloc((void**)&pair_id, ident.size() * sizeof(int)));
-        COTR_CHECK_CUDA(cudaMemcpy(pair_id, ident.data(), ident.size() * sizeof(int), cudaMemcpyHostToDevice));
+        int* pair_id = nullptr;
+        if (mem.upload((void**)&pair_id, ident.data(), ident.size() * sizeof(int))) return 1;
         p.a_pairs = pair_id;
     }
     if (residual_dev) {
@@ -1819,47 +1828,32 @@ int cotr_test_gemm(const cotr_test_gemm_desc* d, const float* A_dev, const float
     if (f32_out) p.out_f32 = out_dev;
     else { if (out16.empty((size_t)d->M * d->N)) return 1; p.out = out16.t; }
     float* wd = nullptr;
-    void* wtc = nullptr;
-    float* scratch = nullptr;
-    const size_t wn = (size_t)d->N * K;
-    COTR_CHECK_CUDA(cudaMalloc((void**)&wd, wn * sizeof(float)));
-    COTR_CHECK_CUDA(cudaMemcpy(wd, w_host, wn * sizeof(float), cudaMemcpyHostToDevice));
+    if (mem.upload((void**)&wd, w_host, (size_t)d->N * K * sizeof(float))) return 1;
+    p.Wt = wd;
     // deferred LayerNorm of A: the packed weights carry gamma, column sums and beta W^T + bias go to the epilogue
-    std::vector<float> w_fold;
-    float *cs_dev = nullptr, *cb_dev = nullptr;
-    float2 *stats_dev = nullptr, *res_stats_dev = nullptr;
+    LnFold fold;
     if (d->a_ln) {
         COTR_CHECK(d->K == 256 && d->a_mode == A_ROWMAJOR, "cotr_test_gemm: a_ln needs K = 256, row-major A");
-        std::vector<float> g(d->K), be(d->K), bias_h(d->N, 0.f), cs(d->N), cb(d->N);
+        std::vector<float> g(d->K), be(d->K), bias_h(d->N, 0.f);
         COTR_CHECK_CUDA(cudaMemcpy(g.data(), ln_gamma_dev, d->K * sizeof(float), cudaMemcpyDeviceToHost));
         COTR_CHECK_CUDA(cudaMemcpy(be.data(), ln_beta_dev, d->K * sizeof(float), cudaMemcpyDeviceToHost));
         if (bias_dev) COTR_CHECK_CUDA(cudaMemcpy(bias_h.data(), bias_dev, d->N * sizeof(float), cudaMemcpyDeviceToHost));
-        w_fold.resize(wn);
-        for (int n = 0; n < d->N; ++n) {
-            double sum = 0.0, c = bias_h[n];
-            for (int k = 0; k < d->K; ++k) {
-                const float v = w_host[(size_t)n * d->K + k] * g[k];
-                w_fold[(size_t)n * d->K + k] = v;
-                sum += v;
-                c += (double)w_host[(size_t)n * d->K + k] * be[k];
-            }
-            cs[n] = (float)sum; cb[n] = (float)c;
-        }
-        COTR_CHECK_CUDA(cudaMalloc((void**)&cs_dev, d->N * sizeof(float)));
-        COTR_CHECK_CUDA(cudaMalloc((void**)&cb_dev, d->N * sizeof(float)));
-        COTR_CHECK_CUDA(cudaMemcpy(cs_dev, cs.data(), d->N * sizeof(float), cudaMemcpyHostToDevice));
-        COTR_CHECK_CUDA(cudaMemcpy(cb_dev, cb.data(), d->N * sizeof(float), cudaMemcpyHostToDevice));
+        fold = fold_ln(w_host, bias_h.data(), d->N, d->K, g.data(), be.data());
+        float *cs_dev = nullptr, *cb_dev = nullptr;
+        float2* stats_dev = nullptr;
+        if (mem.upload((void**)&cs_dev, fold.cs.data(), d->N * sizeof(float)) ||
+            mem.upload((void**)&cb_dev, fold.b.data(), d->N * sizeof(float)) ||
+            mem.alloc((void**)&stats_dev, (size_t)d->M * 16 * sizeof(float2)))
+            return 1;
         p.a_ln_cs = cs_dev; p.bias = cb_dev;
-        w_host = w_fold.data();
-    }
-    if (d->a_ln) {
-        COTR_CHECK_CUDA(cudaMalloc((void**)&stats_dev, (size_t)d->M * 16 * sizeof(float2)));
+        w_host = fold.w.data();
         if (launch_ln_partials(p.a, stats_dev, d->M, 0)) return 1;
         p.a_ln_part = stats_dev;
     }
     if (d->res_ln) {
         COTR_CHECK(residual_dev && d->ldr == 256 && d->N == 256, "cotr_test_gemm: res_ln needs a [M,256] residual");
-        COTR_CHECK_CUDA(cudaMalloc((void**)&res_stats_dev, (size_t)d->M * 16 * sizeof(float2)));
+        float2* res_stats_dev = nullptr;
+        if (mem.alloc((void**)&res_stats_dev, (size_t)d->M * 16 * sizeof(float2))) return 1;
         if (launch_ln_partials(p.res, res_stats_dev, d->M, 0)) return 1;
         p.res_ln_part = res_stats_dev; p.res_ln_gamma = ln_gamma_dev; p.res_ln_beta = ln_beta_dev;
     }
@@ -1867,12 +1861,9 @@ int cotr_test_gemm(const cotr_test_gemm_desc* d, const float* A_dev, const float
         COTR_CHECK(d->path == 0 && part_out_dev != nullptr && d->N == 256, "cotr_test_gemm: emit_part needs path 0, N = 256 and an output buffer");
         p.ln_part_out = reinterpret_cast<float2*>(part_out_dev);
     }
-    const size_t tcb = tc_weight_bytes(d->N, K);
-    std::vector<uint8_t> img(tcb);
-    p.acc_scale = tc_pack_weight(w_host, d->N, K, img.data());
-    COTR_CHECK_CUDA(cudaMalloc(&wtc, tcb));
-    COTR_CHECK_CUDA(cudaMemcpy(wtc, img.data(), tcb, cudaMemcpyHostToDevice));
-    p.Wt = wd; p.Wtc = wtc;
+    void* wtc = nullptr;
+    if (upload_tc_weight(mem, w_host, d->N, K, &wtc, &p.acc_scale)) return 1;
+    p.Wtc = wtc;
     int rc;
     if (d->path == 0) {
         rc = launch_gemm_tc(p, 0);
@@ -1880,7 +1871,8 @@ int cotr_test_gemm(const cotr_test_gemm_desc* d, const float* A_dev, const float
         const float* g = p.ln_gamma; const float* b = p.ln_beta;
         p.ln_gamma = nullptr; p.ln_beta = nullptr;
         if (g) {
-            rc = cudaMalloc((void**)&scratch, (size_t)d->M * d->N * sizeof(float)) != cudaSuccess;
+            float* scratch = nullptr;
+            rc = mem.alloc((void**)&scratch, (size_t)d->M * d->N * sizeof(float));
             if (!rc) rc = launch_gemm_simt_raw(p, scratch, 0);
             if (!rc) rc = launch_layernorm_f32(scratch, g, b, p.out, p.M, 0);
         } else {
@@ -1889,49 +1881,10 @@ int cotr_test_gemm(const cotr_test_gemm_desc* d, const float* A_dev, const float
     }
     if (!rc && !f32_out) rc = launch_split16_to_f32(cs(out16.t), out_dev, (size_t)d->M * d->N, 0);
     cudaError_t e = cudaDeviceSynchronize();
-    cudaFree(wd);
-    cudaFree(wtc);
-    if (scratch) cudaFree(scratch);
-    if (cs_dev) cudaFree(cs_dev);
-    if (cb_dev) cudaFree(cb_dev);
-    if (stats_dev) cudaFree(stats_dev);
-    if (res_stats_dev) cudaFree(res_stats_dev);
-    if (pair_id) cudaFree(pair_id);
     if (rc) return rc;
     COTR_CHECK(e == cudaSuccess, "cotr_test_gemm: kernel failed: %s", cudaGetErrorString(e));
     return 0;
 }
-
-namespace {
-// Device allocations of one test hook call, freed on every return (cudaFree waits for the work queued on them).
-struct DevAllocs {
-    std::vector<void*> ptrs;
-    ~DevAllocs() { for (void* p : ptrs) cudaFree(p); }
-    int alloc(void** out, size_t bytes) {
-        COTR_CHECK_CUDA(cudaMalloc(out, bytes));
-        ptrs.push_back(*out);
-        return 0;
-    }
-    int upload(void** out, const void* host, size_t bytes) {
-        if (alloc(out, bytes)) return 1;
-        COTR_CHECK_CUDA(cudaMemcpy(*out, host, bytes, cudaMemcpyHostToDevice));
-        return 0;
-    }
-};
-
-// tensor-core image of a host [N,K] weight, as the model uploads it; returns acc_scale in *scale
-int upload_tc_weight(DevAllocs& mem, const float* w_host, int N, int K, void** wtc, float* scale) {
-    std::vector<uint8_t> img(tc_weight_bytes(N, K));
-    *scale = tc_pack_weight(w_host, N, K, img.data());
-    return mem.upload(wtc, img.data(), img.size());
-}
-
-std::vector<float> identity(int n) {
-    std::vector<float> eye((size_t)n * n, 0.f);
-    for (int i = 0; i < n; ++i) eye[(size_t)i * n + i] = 1.f;
-    return eye;
-}
-}  // namespace
 
 // The attention launch as the model makes it (see cotr_test_attention_desc).  K / V reach the kernel in the layout of
 // the chosen schedule, produced by the same epilogue stores as in the model: V transposed by the fp32 SIMT identity
@@ -1983,26 +1936,16 @@ int cotr_test_attention(const cotr_test_attention_desc* d, const float* q_dev, c
     a.nq = d->nq; a.npairs = d->npairs; a.pair0 = d->pair0;
     if (d->operands == 1) {
         float* kv = nullptr;
-        void* wtc = nullptr;
-        float scale = 1.f;
         unsigned char* img = nullptr;
         const size_t img_bytes = (size_t)d->ctx_pairs * d->slots * kHeads * kAttnHeadImgBytes;
-        const std::vector<float> eye = identity(2 * kDModel);
-        if (mem.alloc((void**)&kv, kv_rows * 2 * kDModel * sizeof(float)) || mem.alloc((void**)&img, img_bytes) ||
-            upload_tc_weight(mem, eye.data(), 2 * kDModel, 2 * kDModel, &wtc, &scale)) return 1;
+        if (mem.alloc((void**)&kv, kv_rows * 2 * kDModel * sizeof(float)) || mem.alloc((void**)&img, img_bytes)) return 1;
         COTR_CHECK_CUDA(cudaMemcpy2D(kv, 2 * kDModel * sizeof(float), k_dev + (size_t)d->slot * kDModel, kv_ld * sizeof(float),
                                      kDModel * sizeof(float), kv_rows, cudaMemcpyDeviceToDevice));
         COTR_CHECK_CUDA(cudaMemcpy2D(kv + kDModel, 2 * kDModel * sizeof(float), v_dev + (size_t)d->slot * kDModel, kv_ld * sizeof(float),
                                      kDModel * sizeof(float), kv_rows, cudaMemcpyDeviceToDevice));
         COTR_CHECK_CUDA(cudaMemset(img, 0xFF, img_bytes));
-        if (kv16.from_f32(kv, kv_rows * 2 * kDModel)) return 1;
-        GemmParams p;
-        memset(&p, 0, sizeof(p));
-        p.M = (int)kv_rows; p.N = 2 * kDModel; p.K = 2 * kDModel;
-        p.a = cs(kv16.t); p.a_mode = A_ROWMAJOR; p.lda = 2 * kDModel;
-        p.Wtc = wtc; p.acc_scale = scale; p.add_period = 1;
-        p.remap = 1; p.blk_map[0] = -1000 - d->slot; p.blk_map[1] = -(d->slot + 1); p.n_vt = d->slots; p.kv_img = img; p.ldc = 2 * kDModel;
-        if (launch_gemm_tc(p, 0)) return 1;
+        if (kv16.from_f32(kv, kv_rows * 2 * kDModel) ||
+            write_operand_images(mem, cs(kv16.t), (int)kv_rows, true, d->slot, d->slots, img)) return 1;
         a.kv_img = img + (size_t)d->slot * kHeads * kAttnHeadImgBytes;
         a.img_pair_stride = (size_t)d->slots * kHeads * kAttnHeadImgBytes;
     } else {
@@ -2099,38 +2042,21 @@ int cotr_test_attention_weights(int path, const float* q_dev, const float* k_dev
     a.q = cs(q16.t); a.ldq = kDModel;
     a.out = out_dev; a.out_pair_stride = (size_t)nq * kTokens;
     a.nq = nq; a.npairs = npairs; a.pair0 = 0;
-    unsigned char* img = nullptr;
+    DevAllocs mem;
     int rc = 0;
     if (path == 0) {
-        COTR_CHECK_CUDA(cudaMalloc((void**)&img, (size_t)npairs * kHeads * kAttnHeadImgBytes));
-        std::vector<float> eye((size_t)kDModel * kDModel, 0.f);
-        for (int i = 0; i < kDModel; ++i) eye[(size_t)i * kDModel + i] = 1.f;
-        std::vector<uint8_t> eye_tc(tc_weight_bytes(kDModel, kDModel));
-        const float eye_scale = tc_pack_weight(eye.data(), kDModel, kDModel, eye_tc.data());
-        void* wtc = nullptr;
-        rc = cudaMalloc(&wtc, eye_tc.size()) != cudaSuccess ||
-             cudaMemcpy(wtc, eye_tc.data(), eye_tc.size(), cudaMemcpyHostToDevice) != cudaSuccess ||
-             cudaMemset(img, 0, (size_t)npairs * kHeads * kAttnHeadImgBytes) != cudaSuccess;
-        if (rc) set_error("cotr_test_attention_weights: device allocation failed");
-        if (!rc) {      // the key blocks of the tensor-core GEMM epilogue go into the operand images
-            GemmParams p;
-            memset(&p, 0, sizeof(p));
-            p.M = npairs * kTokens; p.N = kDModel; p.K = kDModel;
-            p.a = cs(k16.t); p.a_mode = A_ROWMAJOR; p.lda = kDModel;
-            p.Wtc = wtc; p.acc_scale = eye_scale; p.add_period = 1;
-            p.remap = 1; p.blk_map[0] = -1000; p.n_vt = 1; p.kv_img = img; p.ldc = kDModel;
-            rc = launch_gemm_tc(p, 0);
-        }
-        cudaDeviceSynchronize();
-        if (wtc) cudaFree(wtc);
+        unsigned char* img = nullptr;
+        const size_t img_bytes = (size_t)npairs * kHeads * kAttnHeadImgBytes;
+        if (mem.alloc((void**)&img, img_bytes)) return 1;
+        COTR_CHECK_CUDA(cudaMemset(img, 0, img_bytes));
+        if (write_operand_images(mem, cs(k16.t), npairs * kTokens, false, 0, 1, img)) return 1;
         a.kv_img = img; a.img_pair_stride = (size_t)kHeads * kAttnHeadImgBytes;
-        if (!rc) rc = launch_attention_weights_tc(a, 0);
+        rc = launch_attention_weights_tc(a, 0);
     } else {
         a.k = cs(k16.t); a.ldk = kDModel;
         rc = launch_attention_weights_simt(a, 0);
     }
     const cudaError_t e = cudaDeviceSynchronize();
-    if (img) cudaFree(img);
     if (rc) return rc;
     COTR_CHECK(e == cudaSuccess, "cotr_test_attention_weights: kernel failed: %s", cudaGetErrorString(e));
     return 0;
