@@ -41,7 +41,7 @@ class LaunchRecord(ctypes.Structure):
 
 
 KERNEL_NAMES = ("gemm_tc", "gemm_simt", "attention_tc", "attention_simt", "layernorm", "maxpool", "query_encode", "stem_canvas", "gemm_mlp",
-                "attention_weights_tc", "attention_weights_simt")
+                "attention_weights_tc", "attention_weights_simt", "match_queries", "match_pixels", "nearest", "mutual")
 
 # name -> (restype, argtypes); every symbol include/cotr_b200.h declares
 _PROTOTYPES = {
@@ -60,6 +60,11 @@ _PROTOTYPES = {
                                                  ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p]),
     "cotr_decode_ragged": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int,
                                           ctypes.c_void_p, ctypes.c_void_p]),
+    "cotr_mutual_nearest": (ctypes.c_int, [ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p, ctypes.c_int,
+                                           ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]),
+    "cotr_match_keypoints": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p,
+                                            ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p,
+                                            ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]),
     "cotr_forward": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p]),
     "cotr_forward_host": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_void_p]),
     "cotr_preprocess": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_void_p, ctypes.c_int,
@@ -210,6 +215,21 @@ class NativeModel:
         check(lib().cotr_decode_ragged(self.handle, ctx.handle, _ptr(queries), ctypes.c_void_p(off.ctypes.data), off.size - 1,
                                        _ptr(pred), self._stream()), "cotr_decode_ragged")
         return pred
+
+    def match_keypoints(self, feat, sizes, kpts, kpt_offsets, pairs, ctx):
+        """Cached features (2,N,256,1024) + (N,2) int (W,H) sizes + packed (sum K_i,2) fp64 device keypoints with N+1 host
+        offsets + (B,2) pairs -> (corr (R,2) fp64, nearest (R,) int32, match (R,2) int32, count (B,) int32) on the device,
+        in the row layout of cotr_match_keypoints; ctx needs room for 2B pairs."""
+        off, pairs, R = _match_layout(kpt_offsets, pairs)
+        sizes = np.ascontiguousarray(sizes, dtype=np.int32)
+        B = pairs.shape[0]
+        corr = torch.empty((R, 2), dtype=torch.float64, device=kpts.device)
+        nearest, match, count = _match_outputs(R, B, kpts.device)
+        check(lib().cotr_match_keypoints(self.handle, _ptr(feat), feat.shape[1], ctypes.c_void_p(sizes.ctypes.data), _ptr(kpts),
+                                         ctypes.c_void_p(off.ctypes.data), ctypes.c_void_p(pairs.ctypes.data), B, ctx.handle,
+                                         _ptr(corr), _ptr(nearest), _ptr(match), _ptr(count), self._stream()), "cotr_match_keypoints")
+        ctx.pairs = 2 * B
+        return corr, nearest, match, count
 
     def encode_context_attention(self, img, ctx, layer_mask):
         """encode_context that also returns the head-averaged attention maps of the encoder layers selected by
@@ -413,6 +433,35 @@ def group_tasks(pts, boxes, batch_size, max_load, device):
                                  ctypes.c_void_p(out.data_ptr() + 8 * n), stream), "cotr_group_tasks")
     host = out.cpu().numpy()
     return host[:n], host[n:2 * n], int(host[2 * n])
+
+
+def _match_layout(kpt_offsets, pairs):
+    """-> (int64 offsets, int32 (B,2) pairs, R rows of the call); R = 0 when the table is malformed (the library reports it)."""
+    off = np.ascontiguousarray(kpt_offsets, dtype=np.int64).reshape(-1)
+    pairs = np.ascontiguousarray(pairs, dtype=np.int32).reshape(-1, 2)
+    n = off.size - 1
+    R = 0
+    if n >= 1 and pairs.size and (pairs >= 0).all() and (pairs < n).all() and (np.diff(off) >= 0).all():
+        R = int(np.diff(off)[pairs].sum())
+    return off, pairs, R
+
+
+def _match_outputs(R, B, device):
+    """nearest (R,), match (R,2), count (B,): int32 device tensors"""
+    return (torch.empty((R,), dtype=torch.int32, device=device), torch.empty((R, 2), dtype=torch.int32, device=device),
+            torch.empty((B,), dtype=torch.int32, device=device))
+
+
+def mutual_nearest(kpts, kpt_offsets, pairs, corr):
+    """Packed (sum K_i,2) fp64 device keypoints with N+1 host offsets + (B,2) pairs + (R,2) fp64 device pixel predictions
+    in the row layout of cotr_mutual_nearest -> (nearest (R,) int32, match (R,2) int32, count (B,) int32) on the device."""
+    off, pairs, R = _match_layout(kpt_offsets, pairs)
+    dev = kpts.device.index if kpts.device.index is not None else torch.cuda.current_device()
+    nearest, match, count = _match_outputs(R, pairs.shape[0], kpts.device)
+    stream = ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+    check(lib().cotr_mutual_nearest(dev, _ptr(kpts), ctypes.c_void_p(off.ctypes.data), off.size - 1, ctypes.c_void_p(pairs.ctypes.data),
+                                    pairs.shape[0], _ptr(corr), _ptr(nearest), _ptr(match), _ptr(count), stream), "cotr_mutual_nearest")
+    return nearest, match, count
 
 
 def rasterize_triangles(tris, H, W):

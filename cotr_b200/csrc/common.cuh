@@ -299,6 +299,27 @@ int launch_stem_canvas(const float* img, bool halves, Split16 canvas, int n_img,
 int launch_f32_to_split16(const float* in, Split16 out, size_t n, cudaStream_t s);
 int launch_split16_to_f32(CSplit16 in, float* out, size_t n, cudaStream_t s);
 
+// Keypoint matching (match.cu, cotr_match_keypoints / cotr_mutual_nearest).  Rows are packed in context order; context
+// 2p = [a_p | b_p] owns the rows of a_p's keypoints, context 2p+1 = [b_p | a_p] those of b_p's.  A tile is up to
+// kMatchTileRows rows of one context; the per-row kernels run one CTA per tile.
+constexpr int kMatchTileRows = 64;
+struct MatchTile {
+    int row0, rows;           // packed rows row0 .. row0 + rows - 1
+    int left0;                // packed keypoint of row row0 (the left image's keypoints are the rows, in order)
+    int right0, n_right;      // the right image's keypoints: the candidates of nearest
+    int w_left, h_left, w_right, h_right;    // image sizes in pixels (match_queries / match_pixels only)
+    int pad[3];
+};
+static_assert(sizeof(MatchTile) == 3 * sizeof(int4), "match tiles travel in an int4 table");
+// queries[r] = fp32(kp.x / (2 W_left)), fp32(kp.y / H_left), divisions in fp64
+int launch_match_queries(const MatchTile* tiles, int n_tiles, const double* kpts, float* queries, cudaStream_t s);
+// corr[r] = fp64(fp32((p.x - 0.5) * 2)) * W_right, fp64(p.y) * H_right
+int launch_match_pixels(const MatchTile* tiles, int n_tiles, const float* pred, double* corr, cudaStream_t s);
+// nearest[r] = argmin over the right image's keypoints of the fp64 Euclidean distance to corr[r] (-1: no keypoints)
+int launch_nearest(const MatchTile* tiles, int n_tiles, const double* kpts, const double* corr, int* nearest, cudaStream_t s);
+// pairs[p] = (first row of context 2p, rows of context 2p, rows of context 2p+1, 0); one CTA per pair
+int launch_mutual(const int4* pairs, int B, const int* nearest, int* match, int* count, cudaStream_t s);
+
 // Device-side post-processing of the dense pass (dense_post.cu)
 int dense_post_launch(const float* pred, float* out, int n, cudaStream_t s);
 

@@ -95,6 +95,9 @@ struct Workspace {
     // host-buffer entry point staging
     float *img_stage = nullptr, *q_stage = nullptr, *pred_stage = nullptr;
     size_t img_stage_elems = 0, q_stage_elems = 0;
+    // keypoint matching (cotr_match_keypoints): the (rows,2) canvas queries and predictions of one call
+    int64_t cap_match_rows = 0;
+    float *match_q = nullptr, *match_pred = nullptr;
 };
 
 // A host table that reaches the device with one asynchronous copy per call, staged through pinned memory.  `copied` is
@@ -175,6 +178,7 @@ struct cotr_model {
     std::set<long long> shapes_seen;
     cotr::PinnedTable<int> pair_tab;     // cotr_encode_context_pairs: the caller's (B,2) image table
     cotr::PinnedTable<int4> tile_tab;    // cotr_decode_ragged: the attention tile tables of all chunks of a call (AttnParams::tiles)
+    cotr::PinnedTable<int4> match_tab;   // cotr_match_keypoints: the match tiles and pair table of a call (MatchPlan::tab)
     cotr::Preprocessor* pre = nullptr;         // device-side crop / resize / normalise (cotr_preprocess)
     cotr::FlowMerger* merger = nullptr;        // device-side tail of the dense first guess (cotr_flow_tile_merge)
     bool prof_on = false;
@@ -359,7 +363,8 @@ struct Run {
 };
 
 enum KernelId { K_GEMM_TC = 0, K_GEMM_SIMT = 1, K_ATTN_TC = 2, K_ATTN_SIMT = 3, K_LAYERNORM = 4, K_MAXPOOL = 5, K_QENC = 6, K_STEM_CANVAS = 7,
-                K_GEMM_MLP = 8, K_ATTN_WEIGHTS_TC = 9, K_ATTN_WEIGHTS_SIMT = 10 };
+                K_GEMM_MLP = 8, K_ATTN_WEIGHTS_TC = 9, K_ATTN_WEIGHTS_SIMT = 10, K_MATCH_QUERIES = 11, K_MATCH_PIXELS = 12,
+                K_NEAREST = 13, K_MUTUAL = 14 };
 
 // Counts the launch and, when the profiler is on, brackets it with two events on the launching stream.
 struct LaunchScope {
@@ -647,6 +652,11 @@ std::vector<WsBuf> decode_ws_bufs(Workspace& w, int rows) {
             ws_raw(&w.dec_st_a, R * 16), ws_raw(&w.dec_st_b, R * 16)};
 }
 
+// Keypoint matching: the canvas queries and predictions of `rows` packed rows.
+std::vector<WsBuf> match_ws_bufs(Workspace& w, int64_t rows) {
+    return {ws_raw(&w.match_q, (size_t)rows * 2), ws_raw(&w.match_pred, (size_t)rows * 2)};
+}
+
 void ws_release(const std::vector<WsBuf>& bufs) {
     for (const WsBuf& b : bufs) {
         if (b.split) ws_free(b.split);
@@ -768,6 +778,18 @@ int ensure_decode_ws(cotr_model* m, int rows) {
     ws_release(decode_ws_bufs(w, 0));
     if (ws_allocate(decode_ws_bufs(w, rows))) return 1;
     w.cap_rows = rows;
+    return 0;
+}
+
+// Never captured in a graph, so growing it drops none.
+int ensure_match_ws(cotr_model* m, int64_t rows) {
+    Workspace& w = m->ws;
+    if (rows <= w.cap_match_rows) return 0;
+    COTR_CHECK_CUDA(cudaDeviceSynchronize());
+    w.cap_match_rows = 0;     // as in ensure_encode_ws: no stale capacity after a failed allocation
+    ws_release(match_ws_bufs(w, 0));
+    if (ws_allocate(match_ws_bufs(w, rows))) return 1;
+    w.cap_match_rows = rows;
     return 0;
 }
 
@@ -1145,6 +1167,83 @@ int decode_ragged_impl(cotr_model* m, const cotr_context* ctx, const float* quer
     return 0;
 }
 
+// The rows of a matching call (cotr_match_keypoints / cotr_mutual_nearest): context 2p = [a_p | b_p] owns the rows of
+// a_p's keypoints, context 2p+1 = [b_p | a_p] those of b_p's, packed in context order; ctx_off[c] is context c's first
+// row.  `tab` holds the n_tiles match tiles (3 int4 each, common.cuh MatchTile) followed by one (first row of context
+// 2p, rows of 2p, rows of 2p+1, 0) entry per pair for mutual_kernel.  Every argument is checked here, on the host.
+struct MatchPlan {
+    std::vector<int4> tab;
+    std::vector<int64_t> ctx_off;
+    int n_tiles = 0;
+    int64_t rows = 0;
+};
+
+int plan_match(const char* fn, const int64_t* kpt_off, int n_images, const int32_t* pairs, int B, const int32_t* sizes,
+               MatchPlan* plan) {
+    COTR_CHECK(n_images >= 1, "%s: n_images must be >= 1 (got %d)", fn, n_images);
+    COTR_CHECK(B >= 1, "%s: B must be >= 1 (got %d)", fn, B);
+    COTR_CHECK(kpt_off && pairs, "%s: null kpt_offsets_host or pairs_host", fn);
+    COTR_CHECK(kpt_off[0] == 0, "%s: kpt_offsets_host[0] = %lld, must be 0", fn, (long long)kpt_off[0]);
+    for (int i = 0; i < n_images; ++i)
+        COTR_CHECK(kpt_off[i + 1] >= kpt_off[i], "%s: kpt_offsets_host decreases at image %d (%lld -> %lld)", fn, i,
+                   (long long)kpt_off[i], (long long)kpt_off[i + 1]);
+    COTR_CHECK(kpt_off[n_images] <= INT32_MAX, "%s: %lld keypoints in one call (at most %d)", fn, (long long)kpt_off[n_images], INT32_MAX);
+    for (int i = 0; i < 2 * B; ++i)
+        COTR_CHECK(pairs[i] >= 0 && pairs[i] < n_images, "%s: pairs[%d][%d] = %d is outside [0, %d)", fn, i / 2, i % 2,
+                   (int)pairs[i], n_images);
+    if (sizes)
+        for (int i = 0; i < 2 * n_images; ++i)
+            COTR_CHECK(sizes[i] >= 1 && sizes[i] <= 65536, "%s: sizes[%d][%d] = %d is outside [1, 65536]", fn, i / 2, i % 2,
+                       (int)sizes[i]);
+    int64_t R = 0;
+    for (int p = 0; p < B; ++p) R += (kpt_off[pairs[2 * p] + 1] - kpt_off[pairs[2 * p]]) + (kpt_off[pairs[2 * p + 1] + 1] - kpt_off[pairs[2 * p + 1]]);
+    COTR_CHECK(R <= INT32_MAX, "%s: %lld rows in one call (at most %d)", fn, (long long)R, INT32_MAX);
+
+    plan->rows = R;
+    plan->ctx_off.assign(2 * (size_t)B + 1, 0);
+    plan->tab.clear();
+    int64_t row = 0;
+    for (int c = 0; c < 2 * B; ++c) {
+        const int left = pairs[2 * (c / 2) + (c & 1)], right = pairs[2 * (c / 2) + 1 - (c & 1)];
+        const int n_left = (int)(kpt_off[left + 1] - kpt_off[left]);
+        plan->ctx_off[c] = row;
+        for (int i = 0; i < n_left; i += kMatchTileRows) {
+            MatchTile t{};
+            t.row0 = (int)(row + i);
+            t.rows = std::min(kMatchTileRows, n_left - i);
+            t.left0 = (int)kpt_off[left] + i;
+            t.right0 = (int)kpt_off[right];
+            t.n_right = (int)(kpt_off[right + 1] - kpt_off[right]);
+            if (sizes) {
+                t.w_left = sizes[2 * left]; t.h_left = sizes[2 * left + 1];
+                t.w_right = sizes[2 * right]; t.h_right = sizes[2 * right + 1];
+            }
+            int4 v[3];
+            memcpy(v, &t, sizeof(t));
+            plan->tab.insert(plan->tab.end(), v, v + 3);
+        }
+        row += n_left;
+    }
+    plan->ctx_off[2 * B] = row;
+    plan->n_tiles = (int)(plan->tab.size() / 3);
+    for (int p = 0; p < B; ++p)
+        plan->tab.push_back(make_int4((int)plan->ctx_off[2 * p], (int)(plan->ctx_off[2 * p + 1] - plan->ctx_off[2 * p]),
+                                      (int)(plan->ctx_off[2 * p + 2] - plan->ctx_off[2 * p + 1]), 0));
+    return 0;
+}
+
+// Output buffers of a matching call with R rows (NULL allowed when R == 0).
+int check_match_outputs(const char* fn, int64_t R, const double* kpts, const double* corr, const int32_t* nearest,
+                        const int32_t* match, const int32_t* count) {
+    COTR_CHECK(count != nullptr, "%s: null count_dev", fn);
+    COTR_CHECK(((uintptr_t)count & 3) == 0, "%s: count_dev is not 4-byte aligned", fn);
+    if (R == 0) return 0;
+    COTR_CHECK(kpts && corr && nearest && match, "%s: null kpts_dev, corr_dev, nearest_dev or match_dev for %lld rows", fn, (long long)R);
+    COTR_CHECK(((uintptr_t)kpts & 7) == 0 && ((uintptr_t)corr & 7) == 0, "%s: kpts_dev or corr_dev is not 8-byte aligned", fn);
+    COTR_CHECK(((uintptr_t)nearest & 3) == 0 && ((uintptr_t)match & 3) == 0, "%s: nearest_dev or match_dev is not 4-byte aligned", fn);
+    return 0;
+}
+
 // ----------------------------------------------------------------------------------------------
 // model construction
 // ----------------------------------------------------------------------------------------------
@@ -1360,6 +1459,7 @@ void cotr_destroy(cotr_model* m) {
     Workspace& w = m->ws;
     ws_release(encode_ws_bufs(w, 0));
     ws_release(decode_ws_bufs(w, 0));
+    ws_release(match_ws_bufs(w, 0));
     for (float** b : {&w.img_stage, &w.q_stage, &w.pred_stage}) ws_free_f32(b);
     if (m->host_stream) cudaStreamDestroy(m->host_stream);
     for (auto& kv : m->graphs) cudaGraphExecDestroy(kv.second);
@@ -1637,6 +1737,78 @@ int cotr_group_tasks(int device, const double* pts_dev, const double* box_dev, i
                      int32_t* rank_dev, int32_t* n_squads_dev, void* cuda_stream) {
     COTR_CHECK_CUDA(cudaSetDevice(device));
     return group_tasks_launch(pts_dev, box_dev, n, batch_size, max_load, squad_dev, rank_dev, n_squads_dev, (cudaStream_t)cuda_stream);
+}
+
+int cotr_mutual_nearest(int device, const double* kpts_dev, const int64_t* kpt_offsets_host, int n_images, const int32_t* pairs_host,
+                        int B, const double* corr_dev, int32_t* nearest_dev, int32_t* match_dev, int32_t* count_dev, void* cuda_stream) {
+    const char* fn = "cotr_mutual_nearest";
+    MatchPlan plan;
+    if (plan_match(fn, kpt_offsets_host, n_images, pairs_host, B, nullptr, &plan)) return 1;
+    if (check_match_outputs(fn, plan.rows, kpts_dev, corr_dev, nearest_dev, match_dev, count_dev)) return 1;
+    COTR_CHECK_CUDA(cudaSetDevice(device));
+    cudaStream_t s = (cudaStream_t)cuda_stream;
+    // No model, so no persistent staging: the tables live in stream-ordered memory for the duration of the call, copied
+    // from pageable host memory (the runtime may wait for the stream to stage that copy; see the header).
+    const size_t bytes = plan.tab.size() * sizeof(int4);
+    int4* tab = nullptr;
+    COTR_CHECK_CUDA(cudaMallocAsync((void**)&tab, bytes, s));
+    int rc = 0;
+    const cudaError_t e = cudaMemcpyAsync(tab, plan.tab.data(), bytes, cudaMemcpyHostToDevice, s);
+    if (e != cudaSuccess) { set_error("%s: table upload failed: %s", fn, cudaGetErrorString(e)); rc = 1; }
+    if (!rc) rc = launch_nearest(reinterpret_cast<const MatchTile*>(tab), plan.n_tiles, kpts_dev, corr_dev, nearest_dev, s);
+    if (!rc) rc = launch_mutual(tab + 3 * (size_t)plan.n_tiles, B, nearest_dev, match_dev, count_dev, s);
+    cudaFreeAsync(tab, s);
+    return rc;
+}
+
+int cotr_match_keypoints(cotr_model* m, const void* feat_dev, int n_images, const int32_t* sizes_host, const double* kpts_dev,
+                         const int64_t* kpt_offsets_host, const int32_t* pairs_host, int B, cotr_context* ctx, double* corr_dev,
+                         int32_t* nearest_dev, int32_t* match_dev, int32_t* count_dev, void* cuda_stream) {
+    const char* fn = "cotr_match_keypoints";
+    COTR_CHECK(m != nullptr, "%s: null model", fn);
+    m->launches = 0;
+    COTR_CHECK(feat_dev && sizes_host, "%s: null feat_dev or sizes_host", fn);
+    COTR_CHECK(((uintptr_t)feat_dev & 15) == 0, "%s: feat_dev is not 16-byte aligned", fn);
+    COTR_CHECK(ctx && ctx->model == m, "%s: context does not belong to this model", fn);
+    MatchPlan plan;
+    if (plan_match(fn, kpt_offsets_host, n_images, pairs_host, B, sizes_host, &plan)) return 1;
+    COTR_CHECK(2 * (int64_t)B <= ctx->max_pairs, "%s: B = %d pairs need %d contexts, the context holds at most %d", fn, B,
+               2 * B, ctx->max_pairs);
+    if (check_match_outputs(fn, plan.rows, kpts_dev, corr_dev, nearest_dev, match_dev, count_dev)) return 1;
+    COTR_CHECK_CUDA(cudaSetDevice(m->device));
+    cudaStream_t s = (cudaStream_t)cuda_stream;
+    CallOrder order(m, s);
+    // 1. the contexts [a_p | b_p], [b_p | a_p]
+    std::vector<int32_t> ctx_pairs(4 * (size_t)B);
+    for (int p = 0; p < B; ++p) {
+        ctx_pairs[4 * p] = ctx_pairs[4 * p + 3] = pairs_host[2 * p];
+        ctx_pairs[4 * p + 1] = ctx_pairs[4 * p + 2] = pairs_host[2 * p + 1];
+    }
+    if (encode_pairs_impl(m, feat_dev, n_images, ctx_pairs.data(), 2 * B, ctx, s, AttnMaps())) return 1;
+    if (ensure_match_ws(m, plan.rows)) return 1;
+    if (m->match_tab.upload(plan.tab.data(), plan.tab.size(), s)) return 1;
+    const MatchTile* tiles = reinterpret_cast<const MatchTile*>(m->match_tab.dev);
+    const int4* pair_tab = m->match_tab.dev + 3 * (size_t)plan.n_tiles;
+    Workspace& w = m->ws;
+    Run r{m, s};
+    const int R = (int)plan.rows;
+    if (R > 0) {
+        // 2. - 4. keypoints -> canvas queries -> ragged decode -> pixels of the right image
+        {
+            LaunchScope scope(r, K_MATCH_QUERIES, R, 2, 0);
+            if (launch_match_queries(tiles, plan.n_tiles, kpts_dev, w.match_q, s)) return 1;
+        }
+        if (decode_ragged_impl(m, ctx, w.match_q, plan.ctx_off.data(), 2 * B, w.match_pred, s)) return 1;
+        {
+            LaunchScope scope(r, K_MATCH_PIXELS, R, 2, 0);
+            if (launch_match_pixels(tiles, plan.n_tiles, w.match_pred, corr_dev, s)) return 1;
+        }
+        // 5. cotr_mutual_nearest on the same layout
+        LaunchScope scope(r, K_NEAREST, R, 2, 0);
+        if (launch_nearest(tiles, plan.n_tiles, kpts_dev, corr_dev, nearest_dev, s)) return 1;
+    }
+    LaunchScope scope(r, K_MUTUAL, B, 0, 0);
+    return launch_mutual(pair_tab, B, nearest_dev, match_dev, count_dev, s);
 }
 
 int cotr_rasterize_triangles(int device, const float* tris_dev, int n_tri, int H, int W, float* out_dev, void* cuda_stream) {

@@ -169,6 +169,21 @@ class ImageFeatures:
         self.generation = generation
 
 
+class KeypointMatches:
+    """Per-pair results of COTR.match_keypoints, lists of B device tensors (views of the call's packed outputs):
+    matches[p] (M_p,2) int64 (index into the keypoints of pairs[p][0], index into those of pairs[p][1]), in ascending
+    first index; corrs_ab[p] (K_a,2) / corrs_ba[p] (K_b,2) fp64, where each keypoint of a lands in b / of b in a, in
+    pixels; nearest_ab[p] (K_a,) / nearest_ba[p] (K_b,) int32, the nearest keypoint of the other image (-1 if it has
+    none)."""
+
+    def __init__(self, matches, corrs_ab, corrs_ba, nearest_ab, nearest_ba):
+        self.matches = matches
+        self.corrs_ab = corrs_ab
+        self.corrs_ba = corrs_ba
+        self.nearest_ab = nearest_ab
+        self.nearest_ba = nearest_ba
+
+
 _generations = itertools.count(1)      # process-wide, so that features never match another model's weights
 
 
@@ -202,6 +217,7 @@ class COTR(nn.Module):
         self._native = None
         self._ctx_cache = {}
         self._hook_ctx = None                     # context of hooked forwards (grown to the largest batch seen)
+        self._match_ctx = None                    # context of match_keypoints (grown to the largest 2B seen)
         self._generation = next(_generations)     # the weights ImageFeatures were made with
 
     # ---- native handle management ---------------------------------------------------------------------
@@ -210,9 +226,10 @@ class COTR(nn.Module):
         for ctx in self._ctx_cache.values():
             ctx.close()
         self._ctx_cache = {}
-        if self._hook_ctx is not None:
-            self._hook_ctx.close()
-        self._hook_ctx = None
+        for c in (self._hook_ctx, self._match_ctx):
+            if c is not None:
+                c.close()
+        self._hook_ctx = self._match_ctx = None
         if self._native is not None:
             self._native.close()
         self._native = None
@@ -380,8 +397,21 @@ class COTR(nn.Module):
     def encode_context_pairs(self, features, pairs, reuse=False):
         """The Context of the canvases [image pairs[p][0] | image pairs[p][1]] from cached ImageFeatures; `pairs` is a
         (B,2) integer tensor, array or list.  `reuse` and the encoder attention hooks work as in encode_context."""
+        p32 = self._pair_table("encode_context_pairs", features, pairs)
+        ctx = self._context(p32.shape[0], reuse)
+        nat = self.native()
+        enc, _ = self._attention_modules()
+        mask = self._hooked(enc)
+        if not mask:
+            nat.encode_context_pairs(features.tensor, p32, ctx.native)
+        else:
+            self._fire(enc, mask, nat.encode_context_pairs_attention(features.tensor, p32, ctx.native, mask))
+        return ctx
+
+    def _pair_table(self, fn, features, pairs):
+        """Checks that `features` are current and `pairs` is a (B,2) integer table -> int32 numpy (B,2)."""
         if features.generation != self._generation:
-            raise RuntimeError("encode_context_pairs: these ImageFeatures were made with other weights "
+            raise RuntimeError(f"{fn}: these ImageFeatures were made with other weights "
                                "(load_state_dict / .to() / refresh_native since): encode the images again")
         t = features.tensor
         dev = next(self.parameters()).device
@@ -392,16 +422,55 @@ class COTR(nn.Module):
             f"pairs must be a non-empty (B,2) integer table, got shape {p.shape} dtype {p.dtype}"
         p32 = p.astype(np.int32)
         if not np.array_equal(p32, p):
-            raise RuntimeError(f"encode_context_pairs: image index outside [0, {features.n})")
-        ctx = self._context(p32.shape[0], reuse)
-        nat = self.native()
-        enc, _ = self._attention_modules()
-        mask = self._hooked(enc)
-        if not mask:
-            nat.encode_context_pairs(features.tensor, p32, ctx.native)
-        else:
-            self._fire(enc, mask, nat.encode_context_pairs_attention(features.tensor, p32, ctx.native, mask))
-        return ctx
+            raise RuntimeError(f"{fn}: image index outside [0, {features.n})")
+        return p32
+
+    @torch.no_grad()
+    def match_keypoints(self, features, pairs, keypoints, sizes):
+        """Mutual nearest-neighbour matches of keypoints across image pairs, the rule of demo_guided_matching.py:48-62,
+        on the device from cached ImageFeatures (cotr_match_keypoints).  Pair p decodes the keypoints of a = pairs[p][0]
+        in the context [a | b] and those of b = pairs[p][1] in [b | a], with the whole image as the patch (no zoom-in),
+        and keeps (i, j) when b's keypoint j is the nearest to where a's keypoint i lands and a's keypoint i the nearest
+        to where j lands.  keypoints: N (K_i,2) tensors or arrays of (x, y) pixels of the original images (as DISK
+        writes them); sizes: (N,2) original (W, H), each image having been resized whole to 256x256 for encode_images.
+        -> KeypointMatches.  The call makes one device-to-host copy (the B match counts, to split the lists), so it
+        waits for the device.  The decode is ragged, so registered attention hooks are refused (no maps are made)."""
+        p32 = self._pair_table("match_keypoints", features, pairs)
+        enc, dec = self._attention_modules()
+        if self._hooked(enc) or self._hooked(dec):
+            raise RuntimeError("match_keypoints: attention maps are not produced for matching (ragged decode); remove the "
+                               "attention hooks")
+        assert len(keypoints) == features.n, f"keypoints: {len(keypoints)} sets for {features.n} images"
+        dev = next(self.parameters()).device
+        kp = [torch.as_tensor(k, dtype=torch.float64, device=dev) for k in keypoints]    # nested lists too, without fp32
+        for i, k in enumerate(kp):
+            assert k.ndim == 2 and k.shape[1] == 2, f"keypoints: set {i} must be (K,2), got {tuple(k.shape)}"
+        sz = sizes.detach().cpu().numpy() if isinstance(sizes, torch.Tensor) else np.asarray(sizes)
+        assert sz.shape == (features.n, 2), f"sizes must be ({features.n},2) (W, H), got {sz.shape}"
+        sz32 = sz.astype(np.int32)
+        if not np.array_equal(sz32, sz):
+            raise RuntimeError("match_keypoints: image sizes must be integers in [1, 65536]")
+        counts = np.array([k.shape[0] for k in kp], dtype=np.int64)
+        offsets = np.concatenate([[0], np.cumsum(counts)])
+        B = p32.shape[0]
+        if self._match_ctx is None or self._match_ctx.max_pairs < 2 * B:
+            if self._match_ctx is not None:
+                self._match_ctx.close()
+            self._match_ctx = None
+            self._match_ctx = capi.NativeContext(self.native(), 2 * B)
+        packed = torch.cat(kp).contiguous()
+        corr, nearest, match, count = self.native().match_keypoints(features.tensor, sz32, packed, offsets, p32, self._match_ctx)
+        n_match = count.cpu().numpy()
+        rows = counts[p32].reshape(-1)          # rows of contexts 0, 1, ..., 2B-1
+        ctx_off = np.concatenate([[0], np.cumsum(rows)])
+        match = match.long()
+        res = KeypointMatches([], [], [], [], [])
+        for p in range(B):
+            ab, ba, end = int(ctx_off[2 * p]), int(ctx_off[2 * p + 1]), int(ctx_off[2 * p + 2])
+            res.matches.append(match[ab:ab + int(n_match[p])])
+            res.corrs_ab.append(corr[ab:ba]); res.corrs_ba.append(corr[ba:end])
+            res.nearest_ab.append(nearest[ab:ba]); res.nearest_ba.append(nearest[ba:end])
+        return res
 
     @torch.no_grad()
     def decode(self, ctx, queries):

@@ -128,6 +128,41 @@ int cotr_encode_context_pairs(cotr_model* m, const void* feat_dev, int n_images,
 int cotr_decode_ragged(cotr_model* m, const cotr_context* ctx, const float* queries_dev, const int64_t* offsets_host,
                        int B, float* pred_dev, void* cuda_stream);
 
+/* ---- keypoint matching across image pairs ------------------------------------------------------------------------
+ * Guided matching of demo_guided_matching.py:44-62 with the whole image as the patch, on the device.  Images 0..N-1 with
+ * keypoints kpts_dev: fp64 (x, y) pixels, image i's at rows kpt_offsets_host[i] .. kpt_offsets_host[i+1]-1 (N+1 int64,
+ * HOST, starting at 0, never decreasing).  Pair p = (a_p, b_p) = pairs_host[2p], pairs_host[2p+1] (B x 2 int32, HOST)
+ * uses two contexts: 2p = [a_p | b_p] decodes a_p's keypoints and 2p+1 = [b_p | a_p] decodes b_p's.  These rows are packed
+ * in context order, R = sum over p of (K_a + K_b); off_ab[p] = the first row of context 2p.
+ *   query (refinement_task.py:110):       q = fp32(x / (2 W_left)), fp32(y / H_left), divisions in fp64
+ *   pixel (refinement_task.py:145-151):   c = fp64(fp32((p.x - 0.5) * 2)) * W_right, fp64(p.y) * H_right
+ *   nearest (scipy distance_matrix + np.argmin): the index among the right image's keypoints minimising
+ *       d = sqrt(dx dx + dy dy), dx = kp.x - c.x, all fp64 without contraction; equal d (also distinct squared sums whose
+ *       sqrt rounds equal) -> the lowest index; a NaN d wins over any number and the first NaN wins; no keypoints -> -1
+ *   mutual (the demo's double loop): pair p keeps (i, j = nearest_ab[i]) when nearest_ba[j] == i, in ascending i.
+ * Outputs, all DEVICE: corr_dev (R,2) fp64, nearest_dev (R) int32 (an index into the right image's keypoints),
+ * match_dev (R,2) int32 (pair p's matches are rows off_ab[p] .. off_ab[p] + count[p] - 1, (index into kp_a, index into
+ * kp_b)), count_dev (B) int32.  No K_a x K_b buffer exists anywhere.  Every argument is checked on the host before
+ * anything is enqueued.  cotr_match_keypoints stages its tables through the model's pinned buffer (waiting only as
+ * cotr_encode_context_pairs does) and synchronises the device only when its buffers grow; cotr_mutual_nearest has no
+ * model and copies its tables from pageable host memory, so the runtime may wait for the stream while it stages that
+ * copy.  Eager (no CUDA-graph capture). */
+
+/* The matching alone, for predictions made elsewhere (the zoom-in engines): corr_dev (R,2) fp64 pixels in the layout
+ * above -> nearest_dev, match_dev, count_dev.  `device` is the CUDA device index. */
+int cotr_mutual_nearest(int device, const double* kpts_dev, const int64_t* kpt_offsets_host, int n_images,
+                        const int32_t* pairs_host, int B, const double* corr_dev, int32_t* nearest_dev, int32_t* match_dev,
+                        int32_t* count_dev, void* cuda_stream);
+
+/* Cached image features (cotr_encode_images) + pairs + keypoints -> mutual matches, in one call: the encoder tail of the
+ * 2B contexts (as cotr_encode_context_pairs, into ctx, which needs max_pairs >= 2B), the canvas queries, the ragged decode
+ * of cotr_decode_ragged, the pixels written to corr_dev, and cotr_mutual_nearest.  sizes_host: N x 2 int32 (W, H), HOST,
+ * the original image sizes, 1 .. 65536 (each image was resized whole to 256 x 256 for cotr_encode_images).  It launches
+ * the kernels of cotr_encode_context_pairs(2B) + cotr_decode_ragged + 4 (R == 0: + 1, the pair counts). */
+int cotr_match_keypoints(cotr_model* m, const void* feat_dev, int n_images, const int32_t* sizes_host, const double* kpts_dev,
+                         const int64_t* kpt_offsets_host, const int32_t* pairs_host, int B, cotr_context* ctx,
+                         double* corr_dev, int32_t* nearest_dev, int32_t* match_dev, int32_t* count_dev, void* cuda_stream);
+
 /* cotr_encode_context + cotr_decode on an internal context. */
 int cotr_forward(cotr_model* m, const float* img_dev, const float* queries_dev, int B, int Q,
                  float* pred_dev, void* cuda_stream);
@@ -227,8 +262,9 @@ int cotr_last_launch_count(const cotr_model* m);
  * one record per launch in launch order and returns -(count + 1) on success (so 0 records -> -1), > 0 on failure.
  * kernel ids: 0 gemm_tc (wgmma), 1 gemm_simt, 2 attention_tc, 3 attention_simt, 4 layernorm, 5 maxpool,
  * 6 query_encode, 7 stem_canvas, 8 gemm_mlp (fused feed-forward block), 9 attention_weights_tc, 10 attention_weights_simt
- * (the maps of cotr_*_attention).  For GEMMs M,N,K are the problem size; for attention and attention weights
- * M = query rows, N = 512, K = 256. */
+ * (the maps of cotr_*_attention), 11 match_queries, 12 match_pixels, 13 nearest, 14 mutual (cotr_match_keypoints).  For GEMMs
+ * M,N,K are the problem size; for attention and attention weights M = query rows, N = 512, K = 256; for 11-13 M = rows,
+ * N = 2; for 14 M = pairs. */
 typedef struct cotr_launch_record {
     int32_t kernel;
     int32_t M, N, K;
