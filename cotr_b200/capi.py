@@ -22,7 +22,11 @@ class CotrTensor(ctypes.Structure):
 class TestGemmDesc(ctypes.Structure):
     _fields_ = [(n, ctypes.c_int32) for n in (
         "path", "M", "N", "K", "a_mode", "lda", "H", "W", "C", "OH", "OW", "KH", "KW", "stride", "pad",
-        "relu", "add_period", "ld_add", "ldr", "ldc", "a_ln", "res_ln", "emit_part", "reserved")] + [("a_elems", ctypes.c_int64)]
+        "relu", "add_period", "ld_add", "ldr", "ldc", "a_ln", "res_ln", "emit_part", "reserved")] + [("a_elems", ctypes.c_int64)] + \
+        [(n, ctypes.c_int32) for n in ("out_rows", "res_rows", "res_col0", "n_pairs", "n_images", "redirect", "n_vt", "vt_pairs")] + \
+        [("blk_map", ctypes.c_int32 * 12)] + \
+        [(n, ctypes.c_int32) for n in ("force_bn", "force_ksplit", "plan_bn", "plan_loader", "plan_dln", "plan_ksplit",
+                                        "plan_grid_x", "plan_grid_y", "plan_ln_defused", "reserved2")]
 
 
 class TestAttentionDesc(ctypes.Structure):
@@ -90,7 +94,7 @@ _PROTOTYPES = {
     "cotr_profile_end": (ctypes.c_int, [ctypes.c_void_p, ctypes.POINTER(LaunchRecord), ctypes.c_int]),
     "cotr_debug_read": (ctypes.c_int64, [ctypes.c_void_p, ctypes.c_char_p, ctypes.c_void_p, ctypes.c_int64]),
     "cotr_set_gemm_path": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_int]),
-    "cotr_test_gemm": (ctypes.c_int, [ctypes.POINTER(TestGemmDesc)] + [ctypes.c_void_p] * 9),
+    "cotr_test_gemm": (ctypes.c_int, [ctypes.POINTER(TestGemmDesc)] + [ctypes.c_void_p] * 12),
     "cotr_test_attention": (ctypes.c_int, [ctypes.POINTER(TestAttentionDesc)] + [ctypes.c_void_p] * 5),
     "cotr_test_mlp": (ctypes.c_int, [ctypes.POINTER(TestMlpDesc)] + [ctypes.c_void_p] * 10),
     "cotr_test_rowwise": (ctypes.c_int, [ctypes.c_int, ctypes.c_int] + [ctypes.c_void_p] * 6),
@@ -475,37 +479,75 @@ def rasterize_triangles(tris, H, W):
     return out
 
 
-def test_gemm(path, A, w_host, *, bias=None, addmat=None, add_period=1, residual=None, relu=False, ln=None,
-              a_mode=0, conv=None, M=None, ldc=None, a_ln=False, res_ln=False, part_out=None):
-    """Kernel-level hook: out = epilogue(A W^T).  A and optional epilogue operands are CUDA fp32 tensors.
-    a_ln / res_ln: `ln` = (gamma, beta) is a DEFERRED LayerNorm of the A rows / of the residual rows (tensor-core path)."""
+GEMM_LOADERS = ("gather", "im2col", "stem", "halo")
+GEMM_REDIRECT = {None: 0, "vt": 1, "images": 2}
+
+
+def test_gemm(path, A, w_host, *, bias=None, addmat=None, add_period=1, residual=None, res_col0=0, relu=False, ln=None,
+              a_mode=0, conv=None, M=None, ldc=None, out=None, a_ln=False, res_ln=False, part_out=None, pairs=None,
+              n_images=None, blk_map=None, n_vt=0, vt=None, img=None, bn=0, ksplit=0, plan=None):
+    """Kernel-level hook: out = epilogue(A W^T), launched as the model launches it (cotr_test_gemm).
+
+    A: CUDA fp32, contiguous; all of it reaches the kernel (row-major: (rows >= M, lda) with lda >= K, the columns past
+    K must not be read; token gather: (n_images*256, lda) features with `pairs` an (M/512, 2) image table).
+    residual: (rows >= M, ldr), the launch reads columns res_col0 .. res_col0+N-1.  out: (rows >= M, ldc >= N), rows and
+    columns the launch does not write come back as passed (default: zeros of (M, ldc or N)).
+    a_ln / res_ln: `ln` = (gamma, beta) is a DEFERRED LayerNorm of the A rows / of the residual rows (tensor-core path).
+    blk_map (256-column blocks, GemmParams::blk_map) with n_vt slots: values transposed into vt (pairs, n_vt, 256, 512)
+    fp32 (returned updated in place), or keys and values into the operand images `img` (a uint8 CUDA buffer of
+    pairs * n_vt * 8 * 132096 bytes, left undecoded).  bn / ksplit (path 0): force the tile width / split-K, 0 = rule.
+    plan: a dict that receives the plan the launch used (tile width, loader, dln, ksplit, grid, ln_defused)."""
     N, K = w_host.shape
+    assert A.is_cuda and A.dtype == torch.float32 and A.is_contiguous()
     d = TestGemmDesc()
     d.path = path
     d.N, d.K = N, K
     d.a_mode = a_mode
     if a_mode == 0:
         d.M = A.shape[0] if M is None else M
-        d.lda = A.stride(0)
+        d.lda = A.shape[-1]
     else:
         d.M = M
-        for k_, v_ in conv.items():
+        for k_, v_ in (conv or {}).items():
             setattr(d, k_, v_)
         d.lda = conv.get("C", 0) if a_mode != 3 else A.shape[-1]
     d.a_elems = A.numel()
+    tab = None
+    if a_mode == 3:
+        tab = np.ascontiguousarray(np.arange(2 * (d.M // 512)) if pairs is None else pairs, dtype=np.int32).reshape(-1, 2)
+        d.n_pairs = tab.shape[0]
+        d.n_images = A.numel() // (256 * d.lda) if n_images is None else n_images
     d.relu = int(relu)
     d.a_ln = int(a_ln)
     d.res_ln = int(res_ln)
     d.emit_part = int(part_out is not None)
     d.add_period = add_period
     d.ld_add = addmat.stride(0) if addmat is not None else 0
-    d.ldr = residual.stride(0) if residual is not None else 0
-    d.ldc = N if ldc is None else ldc
-    out = torch.zeros((d.M, d.ldc), dtype=torch.float32, device=A.device)
+    if residual is not None:
+        assert residual.is_contiguous()
+        d.ldr, d.res_rows, d.res_col0 = residual.shape[1], residual.shape[0], res_col0
+    if out is None:
+        out = torch.zeros((d.M, N if ldc is None else ldc), dtype=torch.float32, device=A.device)
+    assert out.is_contiguous() and out.dtype == torch.float32
+    d.out_rows, d.ldc = out.shape
+    if blk_map is not None:
+        d.redirect = GEMM_REDIRECT["images" if img is not None else "vt"]
+        d.n_vt = n_vt
+        buf = img if img is not None else vt
+        d.vt_pairs = buf.shape[0] if vt is not None else buf.numel() // (n_vt * 8 * 132096)
+        assert vt is None or (vt.is_contiguous() and tuple(vt.shape[1:]) == (n_vt, 256, 512))
+        assert img is None or (img.dtype == torch.uint8 and img.is_contiguous() and img.numel() == d.vt_pairs * n_vt * 8 * 132096)
+        for i, b in enumerate(blk_map):
+            d.blk_map[i] = b
+    d.force_bn, d.force_ksplit = bn, ksplit
     w_np = np.ascontiguousarray(w_host, np.float32)
     p = lambda t: ctypes.c_void_p(t.data_ptr()) if t is not None else None
     check(lib().cotr_test_gemm(ctypes.byref(d), p(A), ctypes.c_void_p(w_np.ctypes.data), p(bias), p(addmat), p(residual),
-                               p(ln[0]) if ln else None, p(ln[1]) if ln else None, p(out), p(part_out)), "cotr_test_gemm")
+                               p(ln[0]) if ln else None, p(ln[1]) if ln else None, p(out), p(part_out),
+                               ctypes.c_void_p(tab.ctypes.data) if tab is not None else None, p(vt), p(img)), "cotr_test_gemm")
+    if plan is not None:
+        plan.update(bn=d.plan_bn, loader=GEMM_LOADERS[d.plan_loader] if d.plan_bn else None, dln=d.plan_dln,
+                    ksplit=d.plan_ksplit, grid=(d.plan_grid_x, d.plan_grid_y), ln_defused=d.plan_ln_defused)
     return out
 
 

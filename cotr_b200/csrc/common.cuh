@@ -277,6 +277,14 @@ int launch_mlp_tc(const MlpParams& p, cudaStream_t s);
 int launch_gemm_simt_raw(const GemmParams& p, float* raw_out_f32, cudaStream_t s);   // result as plain fp32 [M,N]
 int launch_layernorm_f32(const float* x, const float* gamma, const float* beta, Split16 out, int rows, cudaStream_t s);
 int launch_gemm_tc(const GemmParams& p, cudaStream_t s);
+// The plan of a tensor-core GEMM launch (gemm_tc.cu): tile width (16, 32, 64, or 256 with the LayerNorm epilogue), A
+// loader (0 row-major / token gather, 1 implicit im2col, 2 stem, 3 halo), deferred-LayerNorm instantiation, split-K
+// (CTAs per cluster) and grid.  launch_gemm_tc chooses it by the launch rules; launch_gemm_tc_forced takes the tile width
+// and split-K given (0 = the rule), checks them against the same constraints, and reports the plan it launched.  Test hook.
+struct GemmPlan {
+    int bn, loader, dln, ksplit, grid_x, grid_y;
+};
+int launch_gemm_tc_forced(const GemmParams& p, int bn, int ksplit, GemmPlan* used, cudaStream_t s);
 int launch_attention_simt(const AttnParams& p, cudaStream_t s);
 int launch_attention_tc(const AttnParams& p, cudaStream_t s);
 // launch_mlp_tc / launch_attention_tc with the hidden split (S = 4 or 8 CTAs per row tile) / key split (ks = 1 or 2)

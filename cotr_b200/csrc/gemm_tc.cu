@@ -73,7 +73,7 @@ __host__ __device__ inline int tc_npad(int N) { return N >= 64 ? ((N + 63) / 64)
 // hands each CTA of the cluster whole channel chunks.
 constexpr uint32_t kHaloMaxBytes = 100u * 1024u;        // resident halo tiles of one CTA (both planes, all its chunks)
 constexpr int kHaloMaxChunks = 4;
-constexpr long long kHaloMinCtas = 86;                  // two thirds of the 132 SMs (see launch_one)
+constexpr long long kHaloMinCtas = 86;                  // two thirds of the 132 SMs (see halo_fits)
 __host__ __device__ inline int halo_pitch(const GemmParams& p) { return p.W + 2; }
 __host__ __device__ inline int halo_tiles_per_img(const GemmParams& p) { return (p.OH * halo_pitch(p) + 127) / 128; }
 __host__ __device__ inline int halo_rows(const GemmParams& p) { return 128 + 2 * halo_pitch(p) + 2; }
@@ -616,7 +616,7 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const GemmParams p
                 for (int q = 0; q < kPiecesPerLane; ++q) {
                     const int piece = piece0 + q * 32;
                     const uint4 val = *reinterpret_cast<const uint4*>(wbase + (uint32_t)(plane * 32 + rr) * C::kOutPitch + piece * 16);
-                    if (ok) *reinterpret_cast<uint4*>(gout + roff + piece * 8) = val;
+                    if (ok && n0 + piece * 8 < p.N) *reinterpret_cast<uint4*>(gout + roff + piece * 8) = val;     // the last column tile may pass N
                 }
             }
         };
@@ -766,53 +766,12 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const GemmParams p
     __syncthreads();
 }
 
-template <int BN, bool LN, int MODE, bool DLN = false>
-int launch_one(const GemmParams& p, cudaStream_t s) {
-    using C = Cfg<BN, MODE>;
-    static unsigned long long configured = 0;      // bit per device
-    if (first_use_on_device(&configured)) {
-        COTR_CHECK_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<BN, LN, MODE, DLN>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                             (int)(C::kSmemBytes + C::kPartMaxBytes)));
-    }
-    const int npad = tc_npad(p.N);
-    const int n_img = MODE == LD_HALO ? p.M / (p.OH * p.OW) : 0;
-    dim3 grid(MODE == LD_HALO ? n_img * halo_tiles_per_img(p) : (p.M + C::BM - 1) / C::BM, (p.N + BN - 1) / BN);
-    // Split-K over a thread-block cluster for long reductions on under-filled grids (the K loop is the serial part of
-    // these latency-bound launches): 4 or 2 CTAs per output tile, each >= 4 chunks, at most ~one wave of CTAs.
-    // LD_HALO splits by whole channel chunks, into at most one wave of the 132 SMs (layer2 at one pair: 72 tiles split
-    // by 2 measured 23.4 us against 17.3 us for the im2col launch, its 12 CTAs past the wave running on their own; H100 at 400 W).
-    int ksplit = 1;
-    if constexpr (!LN && BN <= 64 && MODE != LD_STEM4) {
-        const int kc = (p.K + BK - 1) / BK;
-        const int cc = MODE == LD_HALO ? p.C / BK : kc;
-        const long long ctas = (long long)grid.x * grid.y;
-        const long long wave = MODE == LD_HALO ? kNumSms : kWaveCtas;
-        if (!(g_tc_variant & 512) && kc >= (16 >> ((g_tc_variant >> 14) & 3))) {     // bring-up knob: bits 14-15
-            if (C::kMaxSplit >= 4 && kc % 4 == 0 && cc % 4 == 0 && ctas * 4 <= wave) ksplit = 4;
-            else if (C::kMaxSplit >= 2 && kc % 2 == 0 && cc % 2 == 0 && ctas * 2 <= wave) ksplit = 2;
-        }
-    }
-    if constexpr (MODE == LD_HALO) {
-        // The implicit im2col runs the launch when the halo tiles of a CTA's channel chunks do not fit their region, or
-        // when the halo grid would leave a third of the SMs idle (layer2 at one pair: 72 CTAs of 18 chunks measured
-        // 19.0 us against 17.3 us for the 128 im2col CTAs of 9 chunks; layer3's 96 halo CTAs beat its im2col grid).
-        const int ccp = p.C / BK / ksplit;
-        if (ccp > kHaloMaxChunks || (uint32_t)ccp * 2u * halo_plane_bytes(p) > kHaloMaxBytes ||
-            (long long)grid.x * grid.y * ksplit < kHaloMinCtas)
-            return launch_one<BN, LN, LD_CONV>(p, s);
-        COTR_CHECK(p.M == n_img * p.OH * p.OW && p.res.hi == nullptr && p.addmat == nullptr && !p.remap && p.out_f32 == nullptr,
-                   "gemm_tc: the halo loader needs whole images and a plain split16 output");
-    }
-    COTR_CHECK(p.a_ln_cs == nullptr || (DLN && p.K == 256 && p.a_mode == A_ROWMAJOR && p.a_ln_part != nullptr),
-               "gemm_tc: the deferred LayerNorm on A needs a row-major operand with K = 256 and its partial statistics");
-    COTR_CHECK((p.res_ln_part == nullptr && p.ln_part_out == nullptr) || DLN,
-               "gemm_tc: deferred-LayerNorm residual / statistics on an unsupported tile");
-    COTR_CHECK(p.ln_part_out == nullptr || (p.N == 256 && !p.remap && p.out_f32 == nullptr), "gemm_tc: row statistics need a plain N = 256 output");
-    grid.z = ksplit;
-    const size_t smem = C::kSmemBytes + (size_t)(ksplit - 1) * (C::BM / ksplit) * C::kPartPitch;     // incoming partial rows
-    COTR_CHECK_CUDA(launch_kernel_cluster(gemm_tc_kernel<BN, LN, MODE, DLN>, grid, dim3(kThreads), smem, s, ksplit, p, npad));
-    return 0;
-}
+// ---- host side: a plan (tile width, A loader, deferred-LayerNorm instantiation, split-K, grid), then its launch ----
+
+int bm_of(int bn) { return bn >= 256 ? 64 : 128; }
+// Cfg::kMaxSplit, except that the 16-wide tile does not split: the partial rows are XOR-swizzled over 8 16-byte pieces
+// per row, and its rows have 4, so a swizzled piece would land in the next row
+int max_split(int bn) { return bn == 32 || bn == 64 ? 4 : 1; }
 
 // 3x3 stride-1 "same" convolutions over whole images take the halo loader; cotr_debug_set_variant bit 20 keeps them on
 // the implicit im2col (an in-process A/B and the reference of tests/test_conv_halo_gpu.py)
@@ -821,26 +780,139 @@ inline bool halo_conv(const GemmParams& p) {
            (p.C & 63) == 0 && !(g_tc_variant & (1 << 20));
 }
 
-template <int BN, bool LN>
-int launch_mode(const GemmParams& p, cudaStream_t s) {
+// The loader (kernel instantiation) of a tile width; 1 with the error set when none is instantiated.
+int plan_loader(const GemmParams& p, GemmPlan& plan) {
     const bool gather = (p.a_mode == A_ROWMAJOR || p.a_mode == A_TOKENS);
+    plan.dln = 0;
     if (gather && (p.K & 7) == 0 && (p.lda & 7) == 0) {
-        if constexpr (!LN) {
-            const bool dln = p.a_ln_cs != nullptr || p.res_ln_part != nullptr || p.ln_part_out != nullptr;
-            if (dln) return launch_one<BN, LN, LD_GATHER, true>(p, s);
-        }
-        return launch_one<BN, LN, LD_GATHER>(p, s);
+        plan.loader = LD_GATHER;
+        plan.dln = plan.bn < 256 && (p.a_ln_cs != nullptr || p.res_ln_part != nullptr || p.ln_part_out != nullptr);
+        return 0;
     }
-    if constexpr (!LN && BN >= 32) {
-        if (p.a_mode == A_CONV_NHWC && (p.C & 63) == 0) {
-            if (halo_conv(p)) return launch_one<BN, LN, LD_HALO>(p, s);
-            return launch_one<BN, LN, LD_CONV>(p, s);
-        }
+    if (plan.bn >= 32 && plan.bn < 256 && p.a_mode == A_CONV_NHWC && (p.C & 63) == 0) {
+        plan.loader = halo_conv(p) ? LD_HALO : LD_CONV;
+        return 0;
     }
-    if constexpr (!LN && BN == 64) {
-        if (p.a_mode == A_STEM_NHWC4 && p.K == kStemK) return launch_one<64, false, LD_STEM4>(p, s);
+    if (plan.bn == 64 && p.a_mode == A_STEM_NHWC4 && p.K == kStemK) {
+        plan.loader = LD_STEM4;
+        return 0;
     }
-    set_error("gemm_tc: no kernel instantiation for a_mode %d, K %d, lda %d, C %d with tile N %d", p.a_mode, p.K, p.lda, p.C, BN);
+    set_error("gemm_tc: no kernel instantiation for a_mode %d, K %d, lda %d, C %d with tile N %d", p.a_mode, p.K, p.lda, p.C, plan.bn);
+    return 1;
+}
+
+void plan_grid(const GemmParams& p, GemmPlan& plan) {
+    plan.grid_x = plan.loader == LD_HALO ? p.M / (p.OH * p.OW) * halo_tiles_per_img(p) : (p.M + bm_of(plan.bn) - 1) / bm_of(plan.bn);
+    plan.grid_y = (p.N + plan.bn - 1) / plan.bn;
+}
+
+// Split-K over a thread-block cluster for long reductions on under-filled grids (the K loop is the serial part of
+// these latency-bound launches): 4 or 2 CTAs per output tile, each >= 4 chunks, at most ~one wave of CTAs.
+// LD_HALO splits by whole channel chunks, into at most one wave of the 132 SMs (layer2 at one pair: 72 tiles split
+// by 2 measured 23.4 us against 17.3 us for the im2col launch, its 12 CTAs past the wave running on their own; H100 at 400 W).
+int rule_split(const GemmParams& p, const GemmPlan& plan) {
+    if (plan.bn >= 256 || plan.loader == LD_STEM4) return 1;
+    const int kc = (p.K + BK - 1) / BK;
+    const int cc = plan.loader == LD_HALO ? p.C / BK : kc;
+    const long long ctas = (long long)plan.grid_x * plan.grid_y;
+    const long long wave = plan.loader == LD_HALO ? kNumSms : kWaveCtas;
+    if (!(g_tc_variant & 512) && kc >= (16 >> ((g_tc_variant >> 14) & 3))) {     // bring-up knob: bits 14-15
+        if (max_split(plan.bn) >= 4 && kc % 4 == 0 && cc % 4 == 0 && ctas * 4 <= wave) return 4;
+        if (max_split(plan.bn) >= 2 && kc % 2 == 0 && cc % 2 == 0 && ctas * 2 <= wave) return 2;
+    }
+    return 1;
+}
+
+// The implicit im2col runs the launch when the halo tiles of a CTA's channel chunks do not fit their region, or when the
+// halo grid would leave a third of the SMs idle (layer2 at one pair: 72 CTAs of 18 chunks measured 19.0 us against
+// 17.3 us for the 128 im2col CTAs of 9 chunks; layer3's 96 halo CTAs beat its im2col grid).
+bool halo_fits(const GemmParams& p, const GemmPlan& plan) {
+    const int ccp = p.C / BK / plan.ksplit;
+    return ccp <= kHaloMaxChunks && (uint32_t)ccp * 2u * halo_plane_bytes(p) <= kHaloMaxBytes &&
+           (long long)plan.grid_x * plan.grid_y * plan.ksplit >= kHaloMinCtas;
+}
+
+// Split and loader of a plan whose tile width is set: the split rule (or a forced split, 0 = the rule), then the halo
+// fit with its fallback to the im2col loader (which takes the split rule again when it was not forced).
+int plan_split(const GemmParams& p, GemmPlan& plan, int forced_split) {
+    if (plan_loader(p, plan)) return 1;
+    plan_grid(p, plan);
+    const int kc = (p.K + BK - 1) / BK;
+    if (forced_split) {
+        const int ks = forced_split;
+        const int cc = plan.loader == LD_HALO ? p.C / BK : kc;
+        COTR_CHECK(ks == 1 || ks == 2 || ks == 4, "gemm_tc: split-K %d (1, 2 or 4)", ks);
+        COTR_CHECK(ks <= max_split(plan.bn) && (ks == 1 || plan.loader != LD_STEM4),
+                   "gemm_tc: split-K %d on the %d-wide tile with loader %d", ks, plan.bn, plan.loader);
+        COTR_CHECK(kc % ks == 0 && cc % ks == 0, "gemm_tc: split-K %d does not divide %d K chunks (%d channel chunks)", ks, kc, cc);
+    }
+    plan.ksplit = forced_split ? forced_split : rule_split(p, plan);
+    if (plan.loader == LD_HALO && !halo_fits(p, plan)) {
+        plan.loader = LD_CONV;
+        plan_grid(p, plan);
+        if (!forced_split) plan.ksplit = rule_split(p, plan);
+    }
+    return 0;
+}
+
+int check_params(const GemmParams& p) {
+    COTR_CHECK(p.M > 0 && p.N > 0 && p.K > 0, "gemm_tc: empty problem %d x %d x %d", p.M, p.N, p.K);
+    COTR_CHECK(p.Wtc != nullptr, "gemm_tc: weight has no tensor-core image");
+    COTR_CHECK(p.out_f32 != nullptr || (p.N & 15) == 0, "gemm_tc: split16 outputs need N %% 16 == 0 (N=%d)", p.N);
+    COTR_CHECK(p.res.hi == nullptr || ((p.ldr & 15) == 0 && (p.N & 15) == 0 && ((uintptr_t)p.res.hi & 31) == 0 && ((uintptr_t)p.res.lo & 31) == 0),
+               "gemm_tc: residual needs ldr %% 16 == 0 and 32-byte aligned planes");
+    COTR_CHECK(p.addmat == nullptr || ((p.ld_add & 3) == 0 && (p.N & 15) == 0), "gemm_tc: add-matrix needs ld %% 4 == 0");
+    COTR_CHECK(p.out_f32 != nullptr || (p.ldc & 7) == 0, "gemm_tc: split16 output needs ldc %% 8 == 0");
+    if (p.ln_gamma) COTR_CHECK(p.N == 256 && p.relu == 0 && p.out_f32 == nullptr && !p.remap, "gemm_tc: LayerNorm epilogue needs N = 256");
+    return 0;
+}
+
+template <int BN, bool LN, int MODE, bool DLN = false>
+int launch_one(const GemmParams& p, const GemmPlan& plan, cudaStream_t s) {
+    using C = Cfg<BN, MODE>;
+    static unsigned long long configured = 0;      // bit per device
+    if (first_use_on_device(&configured)) {
+        COTR_CHECK_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<BN, LN, MODE, DLN>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                             (int)(C::kSmemBytes + C::kPartMaxBytes)));
+    }
+    const int ksplit = plan.ksplit;
+    const size_t smem = C::kSmemBytes + (size_t)(ksplit - 1) * (C::BM / ksplit) * C::kPartPitch;     // incoming partial rows
+    COTR_CHECK_CUDA(launch_kernel_cluster(gemm_tc_kernel<BN, LN, MODE, DLN>, dim3(plan.grid_x, plan.grid_y, ksplit), dim3(kThreads),
+                                          smem, s, ksplit, p, tc_npad(p.N)));
+    return 0;
+}
+
+int launch_plan(const GemmParams& p, const GemmPlan& plan, cudaStream_t s) {
+    if (plan.loader == LD_HALO)
+        COTR_CHECK(p.M == p.M / (p.OH * p.OW) * p.OH * p.OW && p.res.hi == nullptr && p.addmat == nullptr && !p.remap && p.out_f32 == nullptr,
+                   "gemm_tc: the halo loader needs whole images and a plain split16 output");
+    COTR_CHECK(p.a_ln_cs == nullptr || (plan.dln && p.K == 256 && p.a_mode == A_ROWMAJOR && p.a_ln_part != nullptr),
+               "gemm_tc: the deferred LayerNorm on A needs a row-major operand with K = 256 and its partial statistics");
+    COTR_CHECK((p.res_ln_part == nullptr && p.ln_part_out == nullptr) || plan.dln,
+               "gemm_tc: deferred-LayerNorm residual / statistics on an unsupported tile");
+    COTR_CHECK(p.ln_part_out == nullptr || (p.N == 256 && !p.remap && p.out_f32 == nullptr), "gemm_tc: row statistics need a plain N = 256 output");
+    switch (plan.bn) {
+        case 256:
+            return launch_one<256, true, LD_GATHER>(p, plan, s);
+        case 16:
+            return plan.dln ? launch_one<16, false, LD_GATHER, true>(p, plan, s) : launch_one<16, false, LD_GATHER>(p, plan, s);
+        case 32:
+            switch (plan.loader) {
+                case LD_GATHER: return plan.dln ? launch_one<32, false, LD_GATHER, true>(p, plan, s) : launch_one<32, false, LD_GATHER>(p, plan, s);
+                case LD_CONV: return launch_one<32, false, LD_CONV>(p, plan, s);
+                case LD_HALO: return launch_one<32, false, LD_HALO>(p, plan, s);
+            }
+            break;
+        case 64:
+            switch (plan.loader) {
+                case LD_GATHER: return plan.dln ? launch_one<64, false, LD_GATHER, true>(p, plan, s) : launch_one<64, false, LD_GATHER>(p, plan, s);
+                case LD_CONV: return launch_one<64, false, LD_CONV>(p, plan, s);
+                case LD_HALO: return launch_one<64, false, LD_HALO>(p, plan, s);
+                case LD_STEM4: return launch_one<64, false, LD_STEM4>(p, plan, s);
+            }
+            break;
+    }
+    set_error("gemm_tc: no kernel instantiation for tile N %d with loader %d", plan.bn, plan.loader);
     return 1;
 }
 
@@ -918,21 +990,15 @@ float tc_pack_weight(const float* w, int N, int K, void* dst_host) {
     return ldexpf(1.f, -e);
 }
 
-int launch_gemm_tc(const GemmParams& p, cudaStream_t s) {
-    COTR_CHECK(p.M > 0 && p.N > 0 && p.K > 0, "gemm_tc: empty problem %d x %d x %d", p.M, p.N, p.K);
-    COTR_CHECK(p.Wtc != nullptr, "gemm_tc: weight has no tensor-core image");
-    COTR_CHECK(p.out_f32 != nullptr || (p.N & 15) == 0, "gemm_tc: split16 outputs need N %% 16 == 0 (N=%d)", p.N);
-    COTR_CHECK(p.res.hi == nullptr || ((p.ldr & 15) == 0 && (p.N & 15) == 0 && ((uintptr_t)p.res.hi & 31) == 0 && ((uintptr_t)p.res.lo & 31) == 0),
-               "gemm_tc: residual needs ldr %% 16 == 0 and 32-byte aligned planes");
-    COTR_CHECK(p.addmat == nullptr || ((p.ld_add & 3) == 0 && (p.N & 15) == 0), "gemm_tc: add-matrix needs ld %% 4 == 0");
-    COTR_CHECK(p.out_f32 != nullptr || (p.ldc & 7) == 0, "gemm_tc: split16 output needs ldc %% 8 == 0");
-    if (p.ln_gamma) {
-        COTR_CHECK(p.N == 256 && p.relu == 0 && p.out_f32 == nullptr && !p.remap, "gemm_tc: LayerNorm epilogue needs N = 256");
-        return launch_mode<256, true>(p, s);
-    }
+namespace {
+
+// The tile-width rule.
+int rule_tile(const GemmParams& p, int& bn) {
+    if (p.ln_gamma) { bn = 256; return 0; }
     if (p.N < 64) {
         COTR_CHECK(p.N <= 16, "gemm_tc: N between 17 and 63 is not instantiated");
-        return launch_mode<16, false>(p, s);
+        bn = 16;
+        return 0;
     }
     // Tile width: at small batch most GEMMs of this network have a handful of 128-row tiles, so the 64-wide tile wins
     // once it yields ~86 CTAs (two thirds of the 132 SMs); the 32-wide tile trades tensor efficiency for parallelism
@@ -944,8 +1010,31 @@ int launch_gemm_tc(const GemmParams& p, cudaStream_t s) {
     // bring-up knob (cotr_debug_set_variant): bits 10-11 move the CTA-count threshold of the 64-wide tile
     static const long long kThr[4] = {86, 43, 57, 132};
     const long long thr64 = kThr[(g_tc_variant >> 10) & 3];
-    if (mt * ((p.N + 63) / 64) >= thr64 || p.a_mode == A_STEM_NHWC4 || (p.N % 32) != 0) return launch_mode<64, false>(p, s);
-    return launch_mode<32, false>(p, s);
+    bn = (mt * ((p.N + 63) / 64) >= thr64 || p.a_mode == A_STEM_NHWC4 || (p.N % 32) != 0) ? 64 : 32;
+    return 0;
+}
+
+}  // namespace
+
+int launch_gemm_tc(const GemmParams& p, cudaStream_t s) {
+    GemmPlan plan{};
+    if (check_params(p) || rule_tile(p, plan.bn) || plan_split(p, plan, 0)) return 1;
+    return launch_plan(p, plan, s);
+}
+
+int launch_gemm_tc_forced(const GemmParams& p, int bn, int ksplit, GemmPlan* used, cudaStream_t s) {
+    GemmPlan plan{};
+    if (check_params(p)) return 1;
+    if (bn == 0) {
+        if (rule_tile(p, plan.bn)) return 1;
+    } else {
+        const bool ok = p.ln_gamma ? bn == 256 : (p.N <= 16 ? bn == 16 : (p.N >= 64 && (bn == 64 || (bn == 32 && p.N % 32 == 0))));
+        COTR_CHECK(ok, "gemm_tc: no %d-wide tile for N = %d%s", bn, p.N, p.ln_gamma ? " with the LayerNorm epilogue" : "");
+        plan.bn = bn;
+    }
+    if (plan_split(p, plan, ksplit)) return 1;
+    if (used) *used = plan;
+    return launch_plan(p, plan, s);
 }
 
 }  // namespace cotr

@@ -423,6 +423,11 @@ void redirect_kv(GemmParams& p, int kv0, int slots, int k_col0, Split16 vt, unsi
     p.kv_img = kv_img;
 }
 
+// The fused LayerNorm epilogue needs the whole 256-wide row in one CTA (128 x 256 tile): with few rows that is a
+// handful of CTAs doing a long serial epilogue while the other SMs idle.  Below 64 row tiles the GEMM runs with narrow
+// tiles across many SMs and LayerNorm follows as its own (in-place, one warp per row) kernel.
+inline bool ln_defused(int M) { return (M + 127) / 128 < 64; }
+
 int launch_tc(const Run& r, const GemmParams& p) {
     LaunchScope scope(r, K_GEMM_TC, p.M, p.N, p.K);
     return launch_gemm_tc(p, r.s);
@@ -432,10 +437,7 @@ int launch_tc(const Run& r, const GemmParams& p) {
 int run_gemm(const Run& r, GemmParams p, float* ln_scratch) {
     if (r.m->gemm_path == 0 && p.ln_gamma == nullptr) return launch_tc(r, p);
     if (r.m->gemm_path == 0) {
-        // The fused LayerNorm epilogue needs the whole 256-wide row in one CTA (128 x 256 tile): with few rows that is
-        // a handful of CTAs doing a long serial epilogue while the other SMs idle.  Below ~64 row tiles the GEMM runs
-        // with narrow tiles across many SMs and LayerNorm follows as its own (in-place, one warp per row) kernel.
-        const bool defuse = p.ln_gamma != nullptr && (p.M + 127) / 128 < 64;
+        const bool defuse = p.ln_gamma != nullptr && ln_defused(p.M);
         const float* g = p.ln_gamma;
         const float* b = p.ln_beta;
         if (defuse) { p.ln_gamma = nullptr; p.ln_beta = nullptr; }
@@ -1947,11 +1949,63 @@ int write_operand_images(DevAllocs& mem, CSplit16 kv, int rows, bool values, int
 }
 }  // namespace
 
-int cotr_test_gemm(const cotr_test_gemm_desc* d, const float* A_dev, const float* w_host, const float* bias_dev,
+int cotr_test_gemm(cotr_test_gemm_desc* d, const float* A_dev, const float* w_host, const float* bias_dev,
                    const float* addmat_dev, const float* residual_dev, const float* ln_gamma_dev,
-                   const float* ln_beta_dev, float* out_dev, float* part_out_dev) {
+                   const float* ln_beta_dev, float* out_dev, float* part_out_dev, const int32_t* pairs_host, float* vt_dev,
+                   unsigned char* img_dev) {
     COTR_CHECK(d && A_dev && w_host && out_dev, "cotr_test_gemm: null argument");
-    COTR_CHECK(d->ldc == d->N, "cotr_test_gemm: ldc must equal N");
+    COTR_CHECK(d->path == 0 || d->path == 1, "cotr_test_gemm: path %d (0 tensor cores, 1 fp32 SIMT)", d->path);
+    COTR_CHECK(d->M >= 1 && d->N >= 1 && d->K >= 1, "cotr_test_gemm: empty problem %d x %d x %d", d->M, d->N, d->K);
+    const bool f32_out = (d->N & 15) != 0;
+    const int out_rows = d->out_rows > 0 ? d->out_rows : d->M;
+    COTR_CHECK(out_rows >= d->M, "cotr_test_gemm: out has %d rows, the launch writes %d", out_rows, d->M);
+    COTR_CHECK((d->redirect || d->ldc >= d->N) && (f32_out || d->ldc % 8 == 0),
+               "cotr_test_gemm: ldc %d (>= N = %d without a redirect, a multiple of 8)", d->ldc, d->N);
+    if (d->a_mode == A_ROWMAJOR || d->a_mode == A_TOKENS)
+        COTR_CHECK(d->lda >= d->K, "cotr_test_gemm: lda %d < K %d", d->lda, d->K);
+    if (d->a_mode == A_ROWMAJOR)
+        COTR_CHECK(d->a_elems >= (int64_t)d->M * d->lda, "cotr_test_gemm: A holds %lld elements, %d rows of lda %d need more",
+                   (long long)d->a_elems, d->M, d->lda);
+    if (d->a_mode == A_CONV_NHWC)
+        COTR_CHECK(d->OH > 0 && d->OW > 0 && d->M % (d->OH * d->OW) == 0 &&
+                   d->a_elems >= (int64_t)(d->M / (d->OH * d->OW)) * d->H * d->W * d->C,
+                   "cotr_test_gemm: A holds %lld elements, too few for %d x %d x %d images", (long long)d->a_elems, d->H, d->W, d->C);
+    std::vector<int> pair_tab;
+    if (d->a_mode == A_TOKENS) {
+        // pair p = images (pairs_host[2p], pairs_host[2p+1]) of the (n_images,16,16,lda) features in A
+        COTR_CHECK(d->M % kTokens == 0 && d->n_pairs == d->M / kTokens && pairs_host != nullptr,
+                   "cotr_test_gemm: the token gather needs M = 512 x n_pairs and a pair table (M %d, n_pairs %d)", d->M, d->n_pairs);
+        COTR_CHECK(d->n_images >= 1 && d->a_elems >= (int64_t)d->n_images * 256 * d->lda,
+                   "cotr_test_gemm: A holds %lld elements, too few for %d images of 256 x %d", (long long)d->a_elems, d->n_images, d->lda);
+        pair_tab.assign(pairs_host, pairs_host + 2 * (size_t)d->n_pairs);
+        for (size_t i = 0; i < pair_tab.size(); ++i)
+            COTR_CHECK(pair_tab[i] >= 0 && pair_tab[i] < d->n_images, "cotr_test_gemm: pair %d reads image %d of %d",
+                       (int)(i / 2), pair_tab[i], d->n_images);
+    }
+    const int res_rows = d->res_rows > 0 ? d->res_rows : d->M;
+    if (residual_dev)
+        COTR_CHECK(res_rows >= d->M && d->res_col0 >= 0 && d->res_col0 % 16 == 0 && (int64_t)d->res_col0 + d->N <= d->ldr,
+                   "cotr_test_gemm: residual columns %d .. %d of ldr %d (res_col0 a multiple of 16), %d rows for M = %d",
+                   d->res_col0, d->res_col0 + d->N - 1, d->ldr, res_rows, d->M);
+    COTR_CHECK(d->redirect >= 0 && d->redirect <= 2, "cotr_test_gemm: redirect %d (0 none, 1 transposed values, 2 operand images)", d->redirect);
+    if (d->redirect) {
+        COTR_CHECK(!f32_out && d->N % kDModel == 0 && d->N / kDModel <= 12, "cotr_test_gemm: block redirect needs N a multiple of 256 up to 3072 (N %d)", d->N);
+        COTR_CHECK(d->n_vt >= 1 && d->vt_pairs >= (d->M + kTokens - 1) / kTokens, "cotr_test_gemm: %d slots of %d pairs for M = %d",
+                   d->n_vt, d->vt_pairs, d->M);
+        COTR_CHECK(d->redirect == 1 ? vt_dev != nullptr : (img_dev != nullptr && d->path == 0),
+                   "cotr_test_gemm: redirect %d needs %s", d->redirect, d->redirect == 1 ? "vt" : "the image buffer and path 0");
+        for (int b = 0; b < d->N / kDModel; ++b) {
+            const int m = d->blk_map[b];
+            const bool ok = m >= 0 ? (m % 8 == 0 && (int64_t)m + kDModel <= d->ldc)
+                                   : ((m >= -d->n_vt) || (d->redirect == 2 && m <= -1000 && m > -1000 - d->n_vt));
+            COTR_CHECK(ok, "cotr_test_gemm: blk_map[%d] = %d (ldc %d, %d slots)", b, m, d->ldc, d->n_vt);
+        }
+    } else {
+        COTR_CHECK(vt_dev == nullptr && img_dev == nullptr, "cotr_test_gemm: vt / images without a redirect");
+    }
+    COTR_CHECK(d->force_bn == 0 || d->path == 0, "cotr_test_gemm: a forced plan needs path 0");
+    COTR_CHECK(d->force_ksplit == 0 || d->path == 0, "cotr_test_gemm: a forced plan needs path 0");
+
     GemmParams p;
     memset(&p, 0, sizeof(p));
     p.M = d->M; p.N = d->N; p.K = d->K;
@@ -1962,10 +2016,12 @@ int cotr_test_gemm(const cotr_test_gemm_desc* d, const float* A_dev, const float
     p.ldr = d->ldr; p.relu = d->relu;
     const bool dln = d->a_ln != 0 || d->res_ln != 0;
     COTR_CHECK(!dln || (d->path == 0 && ln_gamma_dev && ln_beta_dev), "cotr_test_gemm: deferred LayerNorm needs path 0 and gamma / beta");
+    const bool out_ln = !dln && ln_gamma_dev != nullptr;
+    COTR_CHECK(!out_ln || (d->N == kDModel && d->ldc == kDModel && !d->redirect), "cotr_test_gemm: the LayerNorm epilogue needs N = ldc = 256");
     if (!dln) { p.ln_gamma = ln_gamma_dev; p.ln_beta = ln_beta_dev; }
     p.ldc = d->ldc;
     DevAllocs mem;
-    TmpSplit a16, res16, out16;
+    TmpSplit a16, res16, out16, vt16;
     int K = d->K;
     std::vector<float> w_stem;
     if (d->a_mode == A_STEM_NHWC4) {
@@ -1982,23 +2038,30 @@ int cotr_test_gemm(const cotr_test_gemm_desc* d, const float* A_dev, const float
         K = kStemK; p.K = K; p.KW = 8; p.C = 4;
     } else {
         COTR_CHECK(d->a_elems > 0, "cotr_test_gemm: a_elems missing");
-        if (a16.from_f32(A_dev, (size_t)d->a_elems)) return 1;
+        if (a16.from_f32(A_dev, (size_t)d->a_elems)) return 1;      // the whole buffer: NaN in its padding reaches the kernel
         p.a = cs(a16.t);
     }
-    if (d->a_mode == A_TOKENS) {            // the canvas order, as cotr_encode_context runs it: pair p = images (2p, 2p+1)
-        std::vector<int> ident(2 * (size_t)((d->M + kTokens - 1) / kTokens));
-        for (size_t i = 0; i < ident.size(); ++i) ident[i] = (int)i;
+    if (d->a_mode == A_TOKENS) {
         int* pair_id = nullptr;
-        if (mem.upload((void**)&pair_id, ident.data(), ident.size() * sizeof(int))) return 1;
+        if (mem.upload((void**)&pair_id, pair_tab.data(), pair_tab.size() * sizeof(int))) return 1;
         p.a_pairs = pair_id;
     }
     if (residual_dev) {
-        if (res16.from_f32(residual_dev, (size_t)d->M * d->ldr)) return 1;
-        p.res = cs(res16.t);
+        if (res16.from_f32(residual_dev, (size_t)res_rows * d->ldr)) return 1;
+        p.res = offset(cs(res16.t), (size_t)d->res_col0);
     }
-    const bool f32_out = (d->N & 15) != 0;
+    // the output buffers are converted in, so everything the launch does not write comes back as it was passed
+    const size_t out_elems = (size_t)out_rows * d->ldc;
+    const size_t vt_elems = d->redirect == 1 ? (size_t)d->vt_pairs * d->n_vt * kVtLayer : 0;
     if (f32_out) p.out_f32 = out_dev;
-    else { if (out16.empty((size_t)d->M * d->N)) return 1; p.out = out16.t; }
+    else { if (out16.from_f32(out_dev, out_elems)) return 1; p.out = out16.t; }
+    if (d->redirect) {
+        p.remap = 1;
+        memcpy(p.blk_map, d->blk_map, sizeof(p.blk_map));
+        p.n_vt = d->n_vt;
+        if (d->redirect == 1) { if (vt16.from_f32(vt_dev, vt_elems)) return 1; p.vt = vt16.t; }
+        else p.kv_img = img_dev;
+    }
     float* wd = nullptr;
     if (mem.upload((void**)&wd, w_host, (size_t)d->N * K * sizeof(float))) return 1;
     p.Wt = wd;
@@ -2019,26 +2082,38 @@ int cotr_test_gemm(const cotr_test_gemm_desc* d, const float* A_dev, const float
             return 1;
         p.a_ln_cs = cs_dev; p.bias = cb_dev;
         w_host = fold.w.data();
+        COTR_CHECK(d->lda == kDModel, "cotr_test_gemm: a_ln needs lda = 256");
         if (launch_ln_partials(p.a, stats_dev, d->M, 0)) return 1;
         p.a_ln_part = stats_dev;
     }
     if (d->res_ln) {
-        COTR_CHECK(residual_dev && d->ldr == 256 && d->N == 256, "cotr_test_gemm: res_ln needs a [M,256] residual");
+        COTR_CHECK(residual_dev && d->ldr == 256 && d->N == 256 && d->res_col0 == 0, "cotr_test_gemm: res_ln needs a [M,256] residual");
         float2* res_stats_dev = nullptr;
         if (mem.alloc((void**)&res_stats_dev, (size_t)d->M * 16 * sizeof(float2))) return 1;
         if (launch_ln_partials(p.res, res_stats_dev, d->M, 0)) return 1;
         p.res_ln_part = res_stats_dev; p.res_ln_gamma = ln_gamma_dev; p.res_ln_beta = ln_beta_dev;
     }
     if (d->emit_part) {
-        COTR_CHECK(d->path == 0 && part_out_dev != nullptr && d->N == 256, "cotr_test_gemm: emit_part needs path 0, N = 256 and an output buffer");
+        COTR_CHECK(d->path == 0 && part_out_dev != nullptr && d->N == 256 && d->ldc == 256, "cotr_test_gemm: emit_part needs path 0, N = ldc = 256 and an output buffer");
         p.ln_part_out = reinterpret_cast<float2*>(part_out_dev);
     }
     void* wtc = nullptr;
     if (upload_tc_weight(mem, w_host, d->N, K, &wtc, &p.acc_scale)) return 1;
     p.Wtc = wtc;
+    d->plan_bn = d->plan_loader = d->plan_dln = d->plan_ksplit = d->plan_grid_x = d->plan_grid_y = d->plan_ln_defused = 0;
     int rc;
     if (d->path == 0) {
-        rc = launch_gemm_tc(p, 0);
+        // the LayerNorm epilogue as run_gemm launches it: fused into the 256-wide tile, or (few rows, or a narrower
+        // tile forced) a narrow-tile GEMM followed by the in-place LayerNorm kernel
+        const bool defuse = out_ln && (d->force_bn ? d->force_bn != 256 : ln_defused(d->M));
+        if (defuse) { p.ln_gamma = nullptr; p.ln_beta = nullptr; }
+        GemmPlan plan{};
+        rc = launch_gemm_tc_forced(p, d->force_bn, d->force_ksplit, &plan, 0);
+        if (!rc && defuse) rc = launch_layernorm(cs(p.out), ln_gamma_dev, ln_beta_dev, p.out, p.M, 0);
+        if (!rc) {
+            d->plan_bn = plan.bn; d->plan_loader = plan.loader; d->plan_dln = plan.dln; d->plan_ksplit = plan.ksplit;
+            d->plan_grid_x = plan.grid_x; d->plan_grid_y = plan.grid_y; d->plan_ln_defused = defuse;
+        }
     } else {
         const float* g = p.ln_gamma; const float* b = p.ln_beta;
         p.ln_gamma = nullptr; p.ln_beta = nullptr;
@@ -2051,7 +2126,8 @@ int cotr_test_gemm(const cotr_test_gemm_desc* d, const float* A_dev, const float
             rc = launch_gemm_simt(p, 0);
         }
     }
-    if (!rc && !f32_out) rc = launch_split16_to_f32(cs(out16.t), out_dev, (size_t)d->M * d->N, 0);
+    if (!rc && !f32_out) rc = launch_split16_to_f32(cs(out16.t), out_dev, out_elems, 0);
+    if (!rc && d->redirect == 1) rc = launch_split16_to_f32(cs(vt16.t), vt_dev, vt_elems, 0);
     cudaError_t e = cudaDeviceSynchronize();
     if (rc) return rc;
     COTR_CHECK(e == cudaSuccess, "cotr_test_gemm: kernel failed: %s", cudaGetErrorString(e));

@@ -298,14 +298,29 @@ typedef struct cotr_test_gemm_desc {
     int32_t res_ln;               /* 1: the residual (ldr = N = 256) is a deferred LayerNorm too, same gamma / beta   */
     int32_t emit_part;            /* 1: also write the [M][16] (mean, M2) partial row statistics of the output (N = 256) */
     int32_t reserved;
-    int64_t a_elems;              /* element count of the A activation tensor (a_mode 0 / 1 / 3)                 */
+    int64_t a_elems;              /* element count of the whole A buffer, all of it converted (a_mode 0 / 1 / 3)    */
+    int32_t out_rows;             /* out is (out_rows >= M, ldc >= N), 0 = M; converted in: what the launch does not write comes back */
+    int32_t res_rows, res_col0;   /* residual buffer (res_rows >= M, 0 = M; ldr); the launch reads columns res_col0 ..      */
+    int32_t n_pairs, n_images;    /* a_mode 3: pairs_host [n_pairs][2] images of A = (n_images,16,16,lda) features, M = 512 n_pairs */
+    int32_t redirect;             /* GemmParams::blk_map: 0 none; 1 values transposed into vt_dev (vt_pairs,n_vt,256,512) fp32,
+                                     converted in and out; 2 keys / values into the operand images img_dev (path 0), raw bytes */
+    int32_t n_vt, vt_pairs;
+    int32_t blk_map[12];
+    int32_t force_bn, force_ksplit;   /* path 0: tile width (16 / 32 / 64 / 256) and split-K (1 / 2 / 4), 0 = launch rule */
+    int32_t plan_bn, plan_loader, plan_dln, plan_ksplit;   /* set by the call on path 0: the plan it launched (loader
+                                     0 gather, 1 im2col, 2 stem, 3 halo; dln: deferred-LayerNorm instantiation)          */
+    int32_t plan_grid_x, plan_grid_y;
+    int32_t plan_ln_defused;      /* 1: the LayerNorm ran as its own kernel after a narrow-tile GEMM (run_gemm's rule)   */
+    int32_t reserved2;
 } cotr_test_gemm_desc;
-/* out = epilogue(A * W^T): A/bias/addmat/residual/ln_* /out are fp32 DEVICE pointers (may be NULL where optional) -
+/* out = epilogue(A * W^T): A/bias/addmat/residual/ln_* /out/vt are fp32 DEVICE pointers (may be NULL where optional) -
  * the hook converts activations to / from the library's split16 storage around the kernel under test; w_host is a HOST
- * [N,K] matrix (packed for the tensor-core path internally). */
-int cotr_test_gemm(const cotr_test_gemm_desc* d, const float* A_dev, const float* w_host, const float* bias_dev,
+ * [N,K] matrix (packed for the tensor-core path internally), pairs_host a HOST int32 table.  Every argument is checked
+ * before anything is launched. */
+int cotr_test_gemm(cotr_test_gemm_desc* d, const float* A_dev, const float* w_host, const float* bias_dev,
                    const float* addmat_dev, const float* residual_dev, const float* ln_gamma_dev,
-                   const float* ln_beta_dev, float* out_dev, float* part_out_dev /* [M][16][2] or NULL */);
+                   const float* ln_beta_dev, float* out_dev, float* part_out_dev /* [M][16][2] or NULL */,
+                   const int32_t* pairs_host, float* vt_dev, unsigned char* img_dev);
 typedef struct cotr_test_attention_desc {
     int32_t path;                 /* 0 = wgmma (attention_tc.cu), 1 = fp32 SIMT (attention_simt.cu)                */
     int32_t nq, npairs;           /* uniform layout: local pair p owns q / out rows p*nq .. p*nq+nq-1             */
