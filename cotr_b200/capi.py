@@ -39,13 +39,19 @@ class TestMlpDesc(ctypes.Structure):
     _fields_ = [(n, ctypes.c_int32) for n in ("M", "rows", "split", "in_place")]
 
 
+class RefineGroup(ctypes.Structure):
+    _fields_ = [("image_from", ctypes.c_int32), ("image_to", ctypes.c_int32), ("first", ctypes.c_int32), ("count", ctypes.c_int32),
+                ("s_from", ctypes.c_double), ("s_to", ctypes.c_double)]
+
+
 class LaunchRecord(ctypes.Structure):
     _fields_ = [("kernel", ctypes.c_int32), ("M", ctypes.c_int32), ("N", ctypes.c_int32), ("K", ctypes.c_int32),
                 ("ms", ctypes.c_float)]
 
 
 KERNEL_NAMES = ("gemm_tc", "gemm_simt", "attention_tc", "attention_simt", "layernorm", "maxpool", "query_encode", "stem_canvas", "gemm_mlp",
-                "attention_weights_tc", "attention_weights_simt", "match_queries", "match_pixels", "nearest", "mutual")
+                "attention_weights_tc", "attention_weights_simt", "match_queries", "match_pixels", "nearest", "mutual",
+                "refine_geometry", "resize_h", "resize_v", "refine_step")
 
 # name -> (restype, argtypes); every symbol include/cotr_b200.h declares
 _PROTOTYPES = {
@@ -73,6 +79,9 @@ _PROTOTYPES = {
     "cotr_forward_host": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_void_p]),
     "cotr_preprocess": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_void_p, ctypes.c_int,
                                        ctypes.c_int, ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p]),
+    "cotr_refine": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p, ctypes.c_int,
+                                   ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int64, ctypes.c_double]
+                    + [ctypes.c_void_p] * 8),
     "cotr_dense_postprocess": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p]),
     "cotr_flow_tile_merge": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p] + [ctypes.c_int] * 6 +
                              [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p]),
@@ -99,6 +108,7 @@ _PROTOTYPES = {
     "cotr_test_mlp": (ctypes.c_int, [ctypes.POINTER(TestMlpDesc)] + [ctypes.c_void_p] * 10),
     "cotr_test_rowwise": (ctypes.c_int, [ctypes.c_int, ctypes.c_int] + [ctypes.c_void_p] * 6),
     "cotr_test_attention_weights": (ctypes.c_int, [ctypes.c_int] + [ctypes.c_void_p] * 3 + [ctypes.c_int, ctypes.c_int]),
+    "cotr_test_refine_math": (ctypes.c_int, [ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_double] + [ctypes.c_void_p] * 4),
     "cotr_debug_set_variant": (None, [ctypes.c_int]),
     "cotr_last_error": (ctypes.c_char_p, []),
     "cotr_version": (ctypes.c_char_p, []),
@@ -297,6 +307,26 @@ class NativeModel:
                                     _ptr(img_to_dev), img_to_dev.shape[0], img_to_dev.shape[1],
                                     ctypes.c_void_p(rects.ctypes.data), n, _ptr(canvas), self._stream()), "cotr_preprocess")
         return canvas
+
+    def refine(self, images, groups, zooms, batch, wave, max_good, rel_threshold, loc_from, loc_to):
+        """The zoom-in walk (cotr_refine).  images: uint8 HWC device tensors; groups: (image_from, image_to, first,
+        count, s_from, s_to) tuples; loc_from / loc_to: (n,2) fp64 device tensors ->
+        (history (n,L+1,2) fp64, rects (n,L,6) int32, good (n,) int32 on the device, walked, (code, chunk, level))."""
+        n, L = loc_from.shape[0], len(zooms)
+        ptrs = (ctypes.c_void_p * len(images))(*[t.data_ptr() for t in images])
+        hw = np.ascontiguousarray([[t.shape[0], t.shape[1]] for t in images], dtype=np.int32)
+        tab = (RefineGroup * len(groups))(*[RefineGroup(*g) for g in groups])
+        z = np.ascontiguousarray(zooms, dtype=np.float64)
+        history = torch.empty((n, L + 1, 2), dtype=torch.float64, device=loc_from.device)
+        rects = torch.empty((n, max(L, 1), 6), dtype=torch.int32, device=loc_from.device)
+        good = torch.zeros((max(n, 1),), dtype=torch.int32, device=loc_from.device)[:n]
+        walked = ctypes.c_int64(0)
+        status = (ctypes.c_int32 * 3)()
+        check(lib().cotr_refine(self.handle, ptrs, ctypes.c_void_p(hw.ctypes.data), len(images), tab, len(groups),
+                                ctypes.c_void_p(z.ctypes.data), L, int(batch), int(wave), int(max_good), float(rel_threshold),
+                                _ptr(loc_from), _ptr(loc_to), _ptr(history), _ptr(rects), _ptr(good), ctypes.byref(walked),
+                                status, self._stream()), "cotr_refine")
+        return history, rects, good, walked.value, tuple(status)
 
     def dense_postprocess(self, pred_dev):
         """(n, 131072, 2) fp32 predictions of the dense grid queries -> (n, 256, 512, 3) [x, y, confidence] (device)."""
@@ -620,3 +650,17 @@ def test_rowwise(op, x, g1=None, b1=None, g2=None, b2=None):
     p = lambda t: _ptr(t) if t is not None else None
     check(lib().cotr_test_rowwise(ROWWISE_OPS[op], x.shape[0], _ptr(x), p(g1), p(b1), p(g2), p(b2), _ptr(out)), "cotr_test_rowwise")
     return out
+
+
+def test_refine_math(op, inputs, ints, levels=1, rel_threshold=0.0):
+    """cotr_test_refine_math: the per-task arithmetic of cotr_refine on the host (see include/cotr_b200.h).
+    op 0 -> (n,4) int32 [left, top, size, flag]; 1 / 2 -> (n,2) float64; 3 -> (n,) int32 good."""
+    a = np.ascontiguousarray(inputs, dtype=np.float64)
+    b = np.ascontiguousarray(ints, dtype=np.int32)
+    n = b.shape[0]
+    out = np.zeros((n, 2), dtype=np.float64)
+    out_i = np.zeros((n, 4 if op == 0 else 1), dtype=np.int32)
+    check(lib().cotr_test_refine_math(int(op), n, int(levels), float(rel_threshold), ctypes.c_void_p(a.ctypes.data),
+                                      ctypes.c_void_p(b.ctypes.data), ctypes.c_void_p(out.ctypes.data),
+                                      ctypes.c_void_p(out_i.ctypes.data)), "cotr_test_refine_math")
+    return out if op in (1, 2) else (out_i if op == 0 else out_i[:, 0])

@@ -350,6 +350,41 @@ Preprocessor* preprocessor_create();
 void preprocessor_destroy(Preprocessor* p);
 int preprocess_launch(Preprocessor* p, const unsigned char* img_from, int hf, int wf, const unsigned char* img_to, int ht, int wt,
                       const int* rects_host, int n, float* canvas_dev, cudaStream_t s);
+// One crop of the resize kernels: side 2i is task i's "from" crop, 2i+1 its "to" crop.
+struct CropSide {
+    const unsigned char* img;   // HWC uint8, 3 channels
+    int img_w;
+    int x, y, size;
+    int ksize;
+    const int* bounds;
+    const int* weights;
+    size_t tmp_offset;          // into the horizontal-pass buffer (bytes)
+};
+// The Pillow coefficient table of a crop side length (built and uploaded on first use, then cached): fills ksize,
+// bounds and weights of `side`.
+int preprocess_coeffs(Preprocessor* p, int size, CropSide* side);
+// The two resize passes over n_sides prepared sides (device table) of side length <= max_size.
+int launch_resize_h(const CropSide* sides, int n_sides, int max_size, unsigned char* tmp, cudaStream_t s);
+int launch_resize_v(const CropSide* sides, int n_sides, const unsigned char* tmp, float* canvas, cudaStream_t s);
+
+// Zoom-in walk of cotr_refine (refine.cu).  One chunk level: the crops of `count` tasks from task0 at one zoom level.
+struct RefineLevel {
+    int task0, count;
+    int level, levels;          // level l of L
+    int chunk;                  // chunk index in the call's walk order
+    CropSide from, to;          // everything but x, y and tmp_offset (set per task by the geometry kernel)
+    int h_from, w_from, h_to, w_to;
+    double thr;                 // rel_threshold * max(h_to, w_to, 3): conclude()'s bound on the history's std
+};
+// get_patch_centered_at's crop side for an h x w image at `scale` (-1 for a NaN scale, where Python raises)
+int refine_crop_size(int h, int w, double scale);
+double refine_threshold(double rel, int h_to, int w_to);
+// task i's crops -> CropSide 2i / 2i+1, rects[(t * L + l) * 6 ..], fp32 canvas query; non-finite positions flag `status`
+int launch_refine_geometry(const RefineLevel& lv, const double* loc_from, const double* history, CropSide* sides,
+                           int32_t* rects, float* queries, unsigned long long* status, cudaStream_t s);
+// predictions -> history row l+1; at the last level the good flag and the chunk's good count; NaN flags `status`
+int launch_refine_step(const RefineLevel& lv, const float* pred, const int32_t* rects, double* history, int32_t* good,
+                       int32_t* chunk_good, unsigned long long* status, cudaStream_t s);
 
 // Bytes of the pre-tiled fp16 hi/lo image of an [N,K] weight matrix, and the host-side packer (returns acc_scale).
 size_t tc_weight_bytes(int N, int K);

@@ -98,6 +98,15 @@ struct Workspace {
     // keypoint matching (cotr_match_keypoints): the (rows,2) canvas queries and predictions of one call
     int64_t cap_match_rows = 0;
     float *match_q = nullptr, *match_pred = nullptr;
+    // zoom-in walk (cotr_refine): one chunk's canvases, crop table, horizontal-pass bytes, queries and predictions, and
+    // the call's status word followed by its per-chunk good counts
+    int cap_refine_tasks = 0;
+    size_t cap_refine_tmp = 0;
+    int64_t cap_refine_chunks = 0;
+    float *refine_canvas = nullptr, *refine_q = nullptr, *refine_pred = nullptr;
+    CropSide* refine_sides = nullptr;
+    unsigned char* refine_tmp = nullptr;
+    unsigned long long* refine_counts = nullptr;
 };
 
 // A host table that reaches the device with one asynchronous copy per call, staged through pinned memory.  `copied` is
@@ -364,7 +373,7 @@ struct Run {
 
 enum KernelId { K_GEMM_TC = 0, K_GEMM_SIMT = 1, K_ATTN_TC = 2, K_ATTN_SIMT = 3, K_LAYERNORM = 4, K_MAXPOOL = 5, K_QENC = 6, K_STEM_CANVAS = 7,
                 K_GEMM_MLP = 8, K_ATTN_WEIGHTS_TC = 9, K_ATTN_WEIGHTS_SIMT = 10, K_MATCH_QUERIES = 11, K_MATCH_PIXELS = 12,
-                K_NEAREST = 13, K_MUTUAL = 14 };
+                K_NEAREST = 13, K_MUTUAL = 14, K_REFINE_GEOMETRY = 15, K_RESIZE_H = 16, K_RESIZE_V = 17, K_REFINE_STEP = 18 };
 
 // Counts the launch and, when the profiler is on, brackets it with two events on the launching stream.
 struct LaunchScope {
@@ -659,6 +668,13 @@ std::vector<WsBuf> match_ws_bufs(Workspace& w, int64_t rows) {
     return {ws_raw(&w.match_q, (size_t)rows * 2), ws_raw(&w.match_pred, (size_t)rows * 2)};
 }
 
+// Zoom-in walk: chunks of `tasks` tasks, `tmp` horizontal-pass bytes, `chunks` per-chunk counters (2 per u64) + status.
+std::vector<WsBuf> refine_ws_bufs(Workspace& w, int tasks, size_t tmp, int64_t chunks) {
+    return {ws_raw(&w.refine_canvas, (size_t)tasks * 3 * COTR_CANVAS_H * COTR_CANVAS_W), ws_raw(&w.refine_q, (size_t)tasks * 2),
+            ws_raw(&w.refine_pred, (size_t)tasks * 2), ws_raw(&w.refine_sides, (size_t)tasks * 2), ws_raw(&w.refine_tmp, tmp),
+            ws_raw(&w.refine_counts, 1 + ((size_t)chunks + 1) / 2)};
+}
+
 void ws_release(const std::vector<WsBuf>& bufs) {
     for (const WsBuf& b : bufs) {
         if (b.split) ws_free(b.split);
@@ -792,6 +808,21 @@ int ensure_match_ws(cotr_model* m, int64_t rows) {
     ws_release(match_ws_bufs(w, 0));
     if (ws_allocate(match_ws_bufs(w, rows))) return 1;
     w.cap_match_rows = rows;
+    return 0;
+}
+
+// Never captured in a graph either; every capacity only grows.
+int ensure_refine_ws(cotr_model* m, int tasks, size_t tmp, int64_t chunks) {
+    Workspace& w = m->ws;
+    if (tasks <= w.cap_refine_tasks && tmp <= w.cap_refine_tmp && chunks <= w.cap_refine_chunks) return 0;
+    tasks = std::max(tasks, w.cap_refine_tasks);
+    tmp = std::max(tmp, w.cap_refine_tmp);
+    chunks = std::max(chunks, w.cap_refine_chunks);
+    COTR_CHECK_CUDA(cudaDeviceSynchronize());
+    w.cap_refine_tasks = 0; w.cap_refine_tmp = 0; w.cap_refine_chunks = 0;    // as in ensure_encode_ws
+    ws_release(refine_ws_bufs(w, 0, 0, 0));
+    if (ws_allocate(refine_ws_bufs(w, tasks, tmp, chunks))) return 1;
+    w.cap_refine_tasks = tasks; w.cap_refine_tmp = tmp; w.cap_refine_chunks = chunks;
     return 0;
 }
 
@@ -1462,6 +1493,7 @@ void cotr_destroy(cotr_model* m) {
     ws_release(encode_ws_bufs(w, 0));
     ws_release(decode_ws_bufs(w, 0));
     ws_release(match_ws_bufs(w, 0));
+    ws_release(refine_ws_bufs(w, 0, 0, 0));
     for (float** b : {&w.img_stage, &w.q_stage, &w.pred_stage}) ws_free_f32(b);
     if (m->host_stream) cudaStreamDestroy(m->host_stream);
     for (auto& kv : m->graphs) cudaGraphExecDestroy(kv.second);
@@ -1669,6 +1701,126 @@ int forward_staged(cotr_model* m, int B, int Q, cudaStream_t s) {
     return forward_eager(m, w.img_stage, w.q_stage, B, Q, w.pred_stage, s);
 }
 
+// The zoom-in walk of cotr_refine, arguments checked.  sizes: n_groups x L x 2 crop sides.  The host loop's batches
+// fall on the chunks: its first `batch` open tasks are the first chunk not yet finished, and after one step each of them
+// is open again one level deeper, so a chunk walks all L levels before the next one starts.  Its good count, and so the
+// max_corrs stop, changes only after a chunk's last level.  Waves only decide how often the host looks at the counts.
+int refine_walk_impl(cotr_model* m, const uint8_t* const* images, const int32_t* hw, const cotr_refine_group* groups, int n_groups,
+                     const std::vector<int>& sizes, int L, int batch, int wave, int64_t max_good, double rel,
+                     const double* loc_from, const double* loc_to, double* history, int32_t* rects, int32_t* good,
+                     int64_t* walked, int32_t* status, cudaStream_t s) {
+    struct Chunk { int group, first, count; };
+    std::vector<Chunk> chunks;
+    size_t tmp = 256;
+    for (int g = 0; g < n_groups; ++g) {
+        const cotr_refine_group& G = groups[g];
+        for (int f = G.first; f < G.first + G.count; f += batch) chunks.push_back({g, f, std::min(batch, G.first + G.count - f)});
+        const size_t rows = (size_t)std::min(batch, G.count);
+        for (int l = 0; l < L; ++l) tmp = std::max(tmp, rows * (sizes[(g * L + l) * 2] + sizes[(g * L + l) * 2 + 1]) * 256 * 3);
+    }
+    const int64_t n = groups[n_groups - 1].first + (int64_t)groups[n_groups - 1].count;
+    const int64_t n_chunks = (int64_t)chunks.size();
+    status[0] = status[1] = status[2] = 0;
+    *walked = 0;
+    if (n == 0 || max_good <= 0) { m->launches = 0; return 0; }
+
+    // the Pillow coefficient tables of every crop side (uploaded once per side length), the per-level crop templates
+    if (!m->pre) m->pre = preprocessor_create();
+    std::vector<RefineLevel> levels((size_t)n_groups * L);
+    for (int g = 0; g < n_groups; ++g) {
+        const cotr_refine_group& G = groups[g];
+        for (int l = 0; l < L; ++l) {
+            RefineLevel& lv = levels[(size_t)g * L + l];
+            lv = RefineLevel();
+            lv.level = l; lv.levels = L;
+            lv.h_from = hw[2 * G.image_from]; lv.w_from = hw[2 * G.image_from + 1];
+            lv.h_to = hw[2 * G.image_to]; lv.w_to = hw[2 * G.image_to + 1];
+            lv.thr = refine_threshold(rel, lv.h_to, lv.w_to);
+            lv.from.img = images[G.image_from]; lv.from.img_w = lv.w_from;
+            lv.to.img = images[G.image_to]; lv.to.img_w = lv.w_to;
+            if (preprocess_coeffs(m->pre, sizes[(g * L + l) * 2], &lv.from)) return 1;
+            if (preprocess_coeffs(m->pre, sizes[(g * L + l) * 2 + 1], &lv.to)) return 1;
+        }
+    }
+    if (ensure_refine_ws(m, std::min<int64_t>(batch, n), tmp, n_chunks)) return 1;
+    Workspace& w = m->ws;
+    int32_t* chunk_good = reinterpret_cast<int32_t*>(w.refine_counts + 1);
+    COTR_CHECK_CUDA(cudaMemsetAsync(w.refine_counts, 0xFF, sizeof(unsigned long long), s));
+    COTR_CHECK_CUDA(cudaMemsetAsync(chunk_good, 0, (size_t)n_chunks * sizeof(int32_t), s));
+    // history row 0 = the first guesses
+    COTR_CHECK_CUDA(cudaMemcpy2DAsync(history, (size_t)(L + 1) * 2 * sizeof(double), loc_to, 2 * sizeof(double), 2 * sizeof(double),
+                                      (size_t)n, cudaMemcpyDeviceToDevice, s));
+
+    Run r{m, s};
+    int launches = 0;
+    const bool look_each_wave = max_good < n;
+    std::vector<int32_t> counts;
+    int64_t good_so_far = 0;
+    for (int64_t w0 = 0; w0 < n_chunks; w0 += wave) {
+        const int64_t w1 = std::min<int64_t>(n_chunks, w0 + wave);
+        for (int64_t c = w0; c < w1; ++c) {
+            const Chunk& ch = chunks[c];
+            for (int l = 0; l < L; ++l) {
+                RefineLevel lv = levels[(size_t)ch.group * L + l];
+                lv.task0 = ch.first; lv.count = ch.count; lv.chunk = (int)c;
+                m->launches = 0;
+                {
+                    LaunchScope scope(r, K_REFINE_GEOMETRY, ch.count, l, 0);
+                    if (launch_refine_geometry(lv, loc_from, history, w.refine_sides, rects, w.refine_q, w.refine_counts, s)) return 1;
+                }
+                {
+                    LaunchScope scope(r, K_RESIZE_H, 2 * ch.count, 0, 0);
+                    if (launch_resize_h(w.refine_sides, 2 * ch.count, std::max(lv.from.size, lv.to.size), w.refine_tmp, s)) return 1;
+                }
+                {
+                    LaunchScope scope(r, K_RESIZE_V, 2 * ch.count, 0, 0);
+                    if (launch_resize_v(w.refine_sides, 2 * ch.count, w.refine_tmp, w.refine_canvas, s)) return 1;
+                }
+                launches += m->launches;
+                if (forward_eager(m, w.refine_canvas, w.refine_q, ch.count, 1, w.refine_pred, s)) return 1;
+                {
+                    LaunchScope scope(r, K_REFINE_STEP, ch.count, l, 0);
+                    if (launch_refine_step(lv, w.refine_pred, rects, history, good, chunk_good, w.refine_counts, s)) return 1;
+                }
+                launches += m->launches;
+            }
+        }
+        m->launches = launches;
+        const bool last = w1 == n_chunks;
+        if (!look_each_wave && !last) continue;
+        // one small copy: the status word, then (when the stop may fall in this wave) the wave's good counts
+        const int64_t n_read = look_each_wave ? w1 - w0 : 0;
+        counts.assign(2 + (size_t)n_read, 0);
+        COTR_CHECK_CUDA(cudaMemcpyAsync(counts.data(), w.refine_counts, sizeof(unsigned long long), cudaMemcpyDeviceToHost, s));
+        if (n_read) COTR_CHECK_CUDA(cudaMemcpyAsync(counts.data() + 2, chunk_good + w0, (size_t)n_read * sizeof(int32_t),
+                                                    cudaMemcpyDeviceToHost, s));
+        COTR_CHECK_CUDA(cudaStreamSynchronize(s));
+        unsigned long long key;
+        memcpy(&key, counts.data(), sizeof(key));
+        int64_t stop = -1;              // the chunk in which the good count reached max_good
+        for (int64_t c = w0; c < w1 && look_each_wave; ++c) {
+            good_so_far += counts[2 + (c - w0)];
+            if (good_so_far >= max_good) { stop = c; break; }
+        }
+        if (key != ~0ull) {
+            const int64_t bad_chunk = (int64_t)(key >> 5);
+            if (stop < 0 || bad_chunk <= stop) {      // the host loop meets it before it stops
+                status[0] = (int32_t)(key & 3);
+                status[1] = (int32_t)bad_chunk;
+                status[2] = (int32_t)((key >> 2) & 7);
+                *walked = chunks[bad_chunk].first;
+                return 0;
+            }
+        }
+        if (stop >= 0) {
+            *walked = chunks[stop].first + (int64_t)chunks[stop].count;
+            return 0;
+        }
+    }
+    *walked = n;
+    return 0;
+}
+
 }  // namespace
 
 int cotr_forward(cotr_model* m, const float* img_dev, const float* queries_dev, int B, int Q, float* pred_dev, void* cuda_stream) {
@@ -1717,6 +1869,53 @@ int cotr_preprocess(cotr_model* m, const uint8_t* img_from_dev, int h_from, int 
     CallOrder order(m, (cudaStream_t)cuda_stream);
     return preprocess_launch(m->pre, img_from_dev, h_from, w_from, img_to_dev, h_to, w_to, rects_host, n, canvas_dev,
                              (cudaStream_t)cuda_stream);
+}
+
+int cotr_refine(cotr_model* m, const uint8_t* const* images_host, const int32_t* hw_host, int n_images,
+                const cotr_refine_group* groups_host, int n_groups, const double* zoom_host, int n_zoom, int batch, int wave,
+                int64_t max_good, double rel_threshold, const double* loc_from_dev, const double* loc_to_dev,
+                double* history_dev, int32_t* rects_dev, int32_t* good_dev, int64_t* walked_host, int32_t* status_host,
+                void* cuda_stream) {
+    const char* fn = "cotr_refine";
+    COTR_CHECK(m != nullptr, "%s: null model", fn);
+    COTR_CHECK(walked_host && status_host, "%s: null walked_host or status_host", fn);
+    COTR_CHECK(images_host && hw_host && groups_host && zoom_host, "%s: null images_host, hw_host, groups_host or zoom_host", fn);
+    COTR_CHECK(n_images >= 1 && n_groups >= 1, "%s: n_images (%d) and n_groups (%d) must be >= 1", fn, n_images, n_groups);
+    COTR_CHECK(n_zoom >= 1 && n_zoom <= 7, "%s: %d zoom levels (1 .. 7: conclude() sums the history sequentially)", fn, n_zoom);
+    COTR_CHECK(batch >= 1 && wave >= 1, "%s: batch (%d) and wave (%d) must be >= 1", fn, batch, wave);
+    for (int i = 0; i < n_images; ++i) {
+        COTR_CHECK(images_host[i] != nullptr, "%s: image %d is null", fn, i);
+        COTR_CHECK(hw_host[2 * i] >= 2 && hw_host[2 * i + 1] >= 2, "%s: image %d is %d x %d", fn, i, hw_host[2 * i], hw_host[2 * i + 1]);
+    }
+    int64_t n = 0;
+    std::vector<int> sizes((size_t)n_groups * n_zoom * 2);
+    for (int g = 0; g < n_groups; ++g) {
+        const cotr_refine_group& G = groups_host[g];
+        COTR_CHECK(G.image_from >= 0 && G.image_from < n_images && G.image_to >= 0 && G.image_to < n_images,
+                   "%s: group %d images (%d, %d) outside [0, %d)", fn, g, G.image_from, G.image_to, n_images);
+        COTR_CHECK(G.count >= 1 && G.first == n, "%s: group %d (first %d, count %d): groups must be non-empty and consecutive from task 0",
+                   fn, g, G.first, G.count);
+        n += G.count;
+        COTR_CHECK(n <= INT32_MAX, "%s: more than %d tasks", fn, INT32_MAX);
+        for (int l = 0; l < n_zoom; ++l)
+            for (int side = 0; side < 2; ++side) {
+                const int img = side ? G.image_to : G.image_from;
+                const int h = hw_host[2 * img], w = hw_host[2 * img + 1];
+                const int size = refine_crop_size(h, w, (side ? G.s_to : G.s_from) * zoom_host[l]);
+                COTR_CHECK(size >= 2 && size <= h && size <= w, "%s: group %d level %d: %s crop side %d in a %d x %d image", fn, g, l,
+                           side ? "to" : "from", size, h, w);
+                sizes[((size_t)g * n_zoom + l) * 2 + side] = size;
+            }
+    }
+    COTR_CHECK(loc_from_dev && loc_to_dev && history_dev && rects_dev && good_dev, "%s: null device buffer", fn);
+    COTR_CHECK(((uintptr_t)loc_from_dev & 7) == 0 && ((uintptr_t)loc_to_dev & 7) == 0 && ((uintptr_t)history_dev & 7) == 0,
+               "%s: loc_from_dev, loc_to_dev or history_dev is not 8-byte aligned", fn);
+    COTR_CHECK(((uintptr_t)rects_dev & 3) == 0 && ((uintptr_t)good_dev & 3) == 0, "%s: rects_dev or good_dev is not 4-byte aligned", fn);
+    COTR_CHECK_CUDA(cudaSetDevice(m->device));
+    cudaStream_t s = (cudaStream_t)cuda_stream;
+    CallOrder order(m, s);
+    return refine_walk_impl(m, images_host, hw_host, groups_host, n_groups, sizes, n_zoom, batch, wave, max_good, rel_threshold,
+                            loc_from_dev, loc_to_dev, history_dev, rects_dev, good_dev, walked_host, status_host, s);
 }
 
 int cotr_dense_postprocess(cotr_model* m, const float* pred_dev, int n, float* out_dev, void* cuda_stream) {

@@ -4,6 +4,7 @@
 // by side and apply to_tensor + ImageNet normalisation -> (n,3,256,512) fp32 canvases ready for cotr_forward.
 // The source images are uploaded once per engine call; per batch only n x 6 integers cross PCIe instead of 50 MB of
 // fp32 canvases, and ~4 ms of single-threaded PIL work per task disappears from the host loop.
+#include <algorithm>
 #include <cmath>
 #include <map>
 #include <vector>
@@ -21,16 +22,6 @@ struct CoeffTable {
     int ksize = 0;
     int* bounds = nullptr;    // device [256][2]: first source index, tap count
     int* weights = nullptr;   // device [256][ksize]
-};
-
-struct CropSide {
-    const unsigned char* img;   // HWC uint8, 3 channels
-    int img_w;
-    int x, y, size;
-    int ksize;
-    const int* bounds;
-    const int* weights;
-    size_t tmp_offset;          // into the horizontal-pass buffer (bytes)
 };
 
 // libImaging/Resample.c precompute_coeffs + normalize_coeffs_8bpc for the bilinear filter (support 1.0), box = whole
@@ -214,6 +205,28 @@ int preprocess_launch(Preprocessor* p, const unsigned char* img_from, int hf, in
     COTR_CHECK_CUDA(cudaGetLastError());
     const dim3 grid_v(kOut * kOut / 256, (unsigned)(2 * n));
     resize_v_normalize_kernel<<<grid_v, 256, 0, s>>>(p->sides_dev, p->tmp, canvas);
+    COTR_CHECK_CUDA(cudaGetLastError());
+    return 0;
+}
+
+int preprocess_coeffs(Preprocessor* p, int size, CropSide* side) {
+    CoeffTable t;
+    if (get_table(p, size, &t)) return 1;
+    side->size = size;
+    side->ksize = t.ksize; side->bounds = t.bounds; side->weights = t.weights;
+    return 0;
+}
+
+int launch_resize_h(const CropSide* sides, int n_sides, int max_size, unsigned char* tmp, cudaStream_t s) {
+    const dim3 grid_h((unsigned)(((size_t)std::max(max_size, kOut) * kOut + 255) / 256), (unsigned)n_sides);
+    resize_h_kernel<<<grid_h, 256, 0, s>>>(sides, tmp);
+    COTR_CHECK_CUDA(cudaGetLastError());
+    return 0;
+}
+
+int launch_resize_v(const CropSide* sides, int n_sides, const unsigned char* tmp, float* canvas, cudaStream_t s) {
+    const dim3 grid_v(kOut * kOut / 256, (unsigned)n_sides);
+    resize_v_normalize_kernel<<<grid_v, 256, 0, s>>>(sides, tmp, canvas);
     COTR_CHECK_CUDA(cudaGetLastError());
     return 0;
 }

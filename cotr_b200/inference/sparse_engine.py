@@ -7,13 +7,17 @@ border / cycle-consistency filters follow the reference so that, driven by the s
 correspondences - including the reference's quirk that the faster engine strands tasks which were never grouped at
 an earlier zoom level (SURVEY.md section 3.3).
 """
+import math
+
 import numpy as np
 import PIL.Image
 import torch
 
-from .inference_helper import THRESHOLD_SPARSE, THRESHOLD_AREA, cotr_flow, cotr_corr_base
+from . import refinement_task
+from .inference_helper import THRESHOLD_SPARSE, THRESHOLD_AREA, cotr_flow, cotr_corr_base, get_patch_centered_at
 from .refinement_task import RefinementTask
 from ..utils import utils
+from ..utils.utils import ImagePatch
 
 
 def stretch_to_square_np(img):
@@ -28,6 +32,22 @@ def _is_open(task, zoom=None):
     return zoom is None or task.cur_zoom == zoom
 
 
+def _is_fresh(task):
+    return (task.status == 'unfinished' and task.result == 'unknown' and not task.submitted and task.cur_zoom_idx == 0
+            and task.cur_iter == 0 and task.total_iter == 0 and len(task.loc_history) == 1 and not task.job_history
+            and not task.all_loc_to_dict and not task.loc_to_at_zoom)
+
+
+def _exact_point(p):
+    """An (x, y) array whose arithmetic in RefinementTask is fp64 arithmetic on its values: float64 and finite, or
+    integers that fp64 holds exactly (Python raises on NaN / inf positions; float32 points compute in float32)."""
+    if not (isinstance(p, np.ndarray) and p.shape == (2,)):
+        return False
+    if p.dtype == np.float64:
+        return bool(np.isfinite(p).all())
+    return p.dtype.kind in 'iu' and bool((np.abs(p.astype(np.float64)) < 2.0 ** 52).all())
+
+
 def _rect_of(task):
     pf, pt = task.cur_job['patch_from'], task.cur_job['patch_to']
     assert pf.w == pf.h and pt.w == pt.h
@@ -35,7 +55,7 @@ def _rect_of(task):
 
 
 class SparseEngine():
-    def __init__(self, model, batch_size, mode='stretching', device_preprocess=True):
+    def __init__(self, model, batch_size, mode='stretching', device_preprocess=True, device_walk=False):
         assert mode in ['stretching', 'tile']
         self.model = model
         self.batch_size = batch_size
@@ -44,6 +64,8 @@ class SparseEngine():
         # When the model is the native one, the crops are resized / normalised on the device (bit-identical to the
         # host PIL path, which remains the behaviour for any other model) - see COTR.preprocess_canvases.
         self.device_preprocess = device_preprocess
+        # device_walk: the single-query loop runs as one device call (COTR.refine_walk) when it can; same results
+        self.device_walk = device_walk
         self._dev_images = {}
 
     # ---- device-side pixels --------------------------------------------------------------------------------
@@ -227,6 +249,9 @@ class SparseEngine():
         first-open search, :201-211, :25-45): quadratic in the task count.  Same decisions and the same printed lines here
         from running counts and a cursor - inside this loop only the tasks of the current batch change state, and a
         task that is not open (finished, already submitted, or at another zoom level) cannot become open again."""
+        if self.device_walk and zoom is None and self._device_walk_fits(tasks):
+            self._device_walk(tasks, max_corrs)
+            return
         num_g, num_f, start = self.num_good_tasks(tasks), self.num_finished_tasks(tasks), 0
         while True:
             print(f'{num_g} / {max_corrs} | {num_f} / {len(tasks)}')
@@ -241,6 +266,79 @@ class SparseEngine():
                 if t.status == 'finished':
                     num_f += 1
                     num_g += t.result == 'good'
+
+    def _device_walk_fits(self, tasks):
+        """The walk's conditions: device pixels, fresh tasks with converge_iters 1, one (s_from, s_to) and one zoom
+        schedule of <= 7 levels, and every crop at least 2 pixels wide (anything else raises in the host loop too)."""
+        if not tasks or not hasattr(self.model, 'refine_walk') or not self._use_device_pixels(tasks):
+            return False
+        first = tasks[0]
+        zooms = list(first.zoom_ins)
+        if not 1 <= len(zooms) <= 7:
+            return False
+        for t in tasks:
+            if not (t.converge_iters == 1 and _is_fresh(t) and t.s_from == first.s_from and t.s_to == first.s_to
+                    and (t.zoom_ins is first.zoom_ins or list(t.zoom_ins) == zooms)
+                    and _exact_point(t.loc_from) and _exact_point(t.cur_loc_to)):
+                return False
+        for z in zooms:
+            for s, img in ((first.s_from, first.image_from), (first.s_to, first.image_to)):
+                scale = s * z
+                if scale != scale or get_patch_centered_at(None, (0, 0), scale, False, img.shape).w < 2:
+                    return False
+        return True
+
+    def _device_walk(self, tasks, max_corrs):
+        """_single_query_loop as one COTR.refine_walk call; every walked task is left exactly as the host loop leaves it,
+        and the same progress lines are printed."""
+        first = tasks[0]
+        n, L, batch = len(tasks), len(first.zoom_ins), self.batch_size
+        max_good = math.ceil(max_corrs) if max_corrs <= n else n
+        image_from, image_to = self._device_image(first.image_from), self._device_image(first.image_to)
+        history, rects, good, walked, (code, chunk, level) = self.model.refine_walk(
+            [image_from, image_to], [(0, 1, 0, n, float(first.s_from), float(first.s_to))], [float(z) for z in first.zoom_ins],
+            batch, max_good, refinement_task.THRESHOLD_PIXELS_RELATIVE, [t.loc_from for t in tasks], [t.cur_loc_to for t in tasks])
+        num_g = num_f = 0
+        for c0 in range(0, walked, batch):
+            for _ in range(L):
+                print(f'{num_g} / {max_corrs} | {num_f} / {n}')
+            c1 = min(c0 + batch, n)
+            num_g += int(good[c0:c1].sum())
+            num_f += c1 - c0
+        self.total_tasks += walked * L
+        if code != 0:
+            for _ in range(level + 1):
+                print(f'{num_g} / {max_corrs} | {num_f} / {n}')
+            self.total_tasks += (min(walked + batch, n) - walked) * (level + 1)
+            raise ValueError('NaN in prediction' if code == 1 else 'non-finite position in the zoom-in walk')
+        print(f'{num_g} / {max_corrs} | {num_f} / {n}')
+        (h_f, w_f), (h_t, w_t) = first.image_from.shape[:2], first.image_to.shape[:2]
+        for i in range(walked):
+            t = tasks[i]
+            for l in range(L):
+                x0, y0, s0, x1, y1, s1 = (int(v) for v in rects[i, l])
+                t.cur_job = {'patch_from': ImagePatch(None, x0, y0, s0, s0, w_f, h_f), 'patch_to': ImagePatch(None, x1, y1, s1, s1, w_t, h_t),
+                             'loc_from': t.loc_from, 'loc_to': t.cur_loc_to, 'img': None}
+                t.job_history.append((s0, s0, s1, s1))
+                # RefinementTask.step + next_zoom with one iteration per level
+                loc = history[i, l + 1].copy()
+                t.total_iter += 1
+                t.loc_to_at_zoom.append(loc)
+                if l == L - 1:
+                    t.cur_iter += 1
+                t.all_loc_to_dict[t.cur_zoom] = np.array(t.loc_to_at_zoom).copy()
+                t.loc_history.append(loc)
+                t.best_loc_to = loc
+                t.cur_loc_to = loc
+                if l == L - 1:
+                    t.status = 'finished'
+                    t.result = 'good' if good[i] else 'bad'
+                t.cur_zoom_idx += 1
+                t.cur_iter = 0
+                t.loc_to_at_zoom = []
+        # the host loop forms (submits) the next batch before it tests max_corrs and stops
+        for t in tasks[walked:walked + batch]:
+            t.get_task_fast()
 
     def _finish(self, tasks, max_corrs, return_idx, force, return_tasks_only, img_a_shape, img_b_shape):
         if return_tasks_only:
@@ -295,8 +393,8 @@ class FasterSparseEngine(SparseEngine):
     """
 
     def __init__(self, model, batch_size, mode='stretching', max_load=256, device_preprocess=True, rescue_stranded=False,
-                 device_grouping=True):
-        super().__init__(model, batch_size, mode=mode, device_preprocess=device_preprocess)
+                 device_grouping=True, device_walk=False):
+        super().__init__(model, batch_size, mode=mode, device_preprocess=device_preprocess, device_walk=device_walk)
         self.max_load = max_load
         self.rescue_stranded = rescue_stranded
         # squads are formed on the device (cotr_group_tasks) whenever the pixels are made there too; the result is

@@ -348,6 +348,25 @@ class COTR(nn.Module):
         return self.native().preprocess(img_from_u8.contiguous(), img_to_u8.contiguous(), rects)
 
     @torch.no_grad()
+    def refine_walk(self, images, groups, zooms, batch, max_good, rel_threshold, loc_from, loc_to, wave=8):
+        """The single-query zoom-in walk of SparseEngine (converge_iters = 1) on the device (cotr_refine).  images: uint8
+        HWC CUDA tensors; groups: (image_from, image_to, first, count, s_from, s_to) per group, consecutive in task order;
+        loc_from / loc_to: (n,2) source points and first guesses (converted to fp64).  Returns (history (n,L+1,2) fp64,
+        rects (n,L,6) int32, good (n,) int32) as numpy arrays, the number of tasks walked and the (code, chunk, level)
+        status (code 1: NaN prediction, 2: non-finite position)."""
+        enc, dec = self._attention_modules()
+        if self._hooked(enc) or self._hooked(dec):
+            raise RuntimeError("refine_walk does not fire attention hooks: remove them or use the host loop")
+        dev = next(self.parameters()).device
+        images = [t.contiguous() for t in images]
+        assert all(t.dtype == torch.uint8 and t.ndim == 3 and t.shape[2] == 3 and t.device == dev for t in images)
+        lf = torch.as_tensor(np.asarray(loc_from, dtype=np.float64).reshape(-1, 2)).to(dev)
+        lt = torch.as_tensor(np.asarray(loc_to, dtype=np.float64).reshape(-1, 2)).to(dev)
+        history, rects, good, walked, status = self.native().refine(images, groups, zooms, batch, wave, max_good,
+                                                                    rel_threshold, lf, lt)
+        return history.cpu().numpy(), rects.cpu().numpy(), good.cpu().numpy(), walked, status
+
+    @torch.no_grad()
     def dense_postprocess(self, pred):
         """Device-side tail of the dense pass (inference_helper.py:131-145): (n,131072,2) predictions of the canvas grid
         queries -> (n,256,512,3) [x in the other image, y, cycle confidence] (cotr_dense_postprocess)."""

@@ -180,6 +180,38 @@ int cotr_forward_host(cotr_model* m, const float* img_host, const float* queries
 int cotr_preprocess(cotr_model* m, const uint8_t* img_from_dev, int h_from, int w_from, const uint8_t* img_to_dev, int h_to,
                     int w_to, const int32_t* rects_host, int n, float* canvas_dev, void* cuda_stream);
 
+/* The single-query zoom-in walk of SparseEngine with converge_iters = 1 (COTR/inference/sparse_engine.py:197-211,
+ * refinement_task.py) on the device, for n fresh tasks.  A group is the tasks first .. first+count-1 of one
+ * (image_from, image_to) pair with one (s_from, s_to); groups are consecutive in task order and cover 0 .. n-1.  The
+ * walk takes chunks of at most `batch` consecutive tasks of one group and walks each chunk through all L = n_zoom levels
+ * before the next, exactly as the host loop's batches fall: per level the crops of get_patch_centered_at (side
+ * min(h, w) * clip(s * zoom_host[l], 0, 1) rounded down to even, known on the host), the canvas query, the Pillow-exact
+ * canvases of cotr_preprocess, the forward of cotr_forward at (chunk, Q = 1), and scale_to_loc; after the last level
+ * conclude(): good when max(std(history, axis=0)) < rel_threshold * max(h_to, w_to, 3).  All of it bit for bit.
+ *   images_host: n_images uint8 HWC (3 channels) DEVICE pointers; hw_host: n_images x 2 (H, W), HOST.
+ *   loc_from_dev, loc_to_dev: n x 2 fp64 (x, y) source points and first guesses, DEVICE.
+ *   history_dev: n x (L+1) x 2 fp64, row 0 = the first guess, row l+1 = the location after level l.
+ *   rects_dev: n x L x 6 int32 [x_from, y_from, size_from, x_to, y_to, size_to] crop of each level.
+ *   good_dev: n int32, 1 when the task is good.
+ * max_good is the engine's max_corrs stop: chunks run in waves of `wave` chunks; after each wave one small copy reads the
+ * good counts (over the whole call, in task order), and the walk ends after the first wave in which they reached
+ * max_good.  *walked_host is then exactly the number of tasks the host loop walks: every task up to the end of the chunk
+ * in which the count reached max_good (n when it never did, 0 when max_good <= 0); later tasks hold no result.  With
+ * max_good >= n the host waits only once, at the end.  status_host: 3 int32 [code, chunk, level]: code 0 ok, 1 a NaN
+ * prediction, 2 a NaN or infinite position (clamped, not used); the walk then ends after the wave, *walked_host is the
+ * first task of that chunk, and the call still returns 0.  Every argument is checked before anything is enqueued
+ * (1 <= L <= 7, every crop side >= 2).  The canvases, crop table, queries and counters are model-owned and grow on demand.
+ * Launches per chunk level: refine_geometry, resize_h, resize_v, the forward, refine_step. */
+typedef struct cotr_refine_group {
+    int32_t image_from, image_to, first, count;
+    double s_from, s_to;
+} cotr_refine_group;
+int cotr_refine(cotr_model* m, const uint8_t* const* images_host, const int32_t* hw_host, int n_images,
+                const cotr_refine_group* groups_host, int n_groups, const double* zoom_host, int n_zoom, int batch, int wave,
+                int64_t max_good, double rel_threshold, const double* loc_from_dev, const double* loc_to_dev,
+                double* history_dev, int32_t* rects_dev, int32_t* good_dev, int64_t* walked_host, int32_t* status_host,
+                void* cuda_stream);
+
 /* Device-side post-processing of the dense first guess (COTR/inference/inference_helper.py:131-145, the host work of
  * cotr_patch_flow_exhaustive after the 131 072-query forward): pred_dev holds n x (256*512) x 2 fp32 predictions for the
  * grid queries (j/512, i/256) in row-major (i, j) order; out_dev receives n x 256 x 512 x 3 fp32
@@ -262,9 +294,10 @@ int cotr_last_launch_count(const cotr_model* m);
  * one record per launch in launch order and returns -(count + 1) on success (so 0 records -> -1), > 0 on failure.
  * kernel ids: 0 gemm_tc (wgmma), 1 gemm_simt, 2 attention_tc, 3 attention_simt, 4 layernorm, 5 maxpool,
  * 6 query_encode, 7 stem_canvas, 8 gemm_mlp (fused feed-forward block), 9 attention_weights_tc, 10 attention_weights_simt
- * (the maps of cotr_*_attention), 11 match_queries, 12 match_pixels, 13 nearest, 14 mutual (cotr_match_keypoints).  For GEMMs
- * M,N,K are the problem size; for attention and attention weights M = query rows, N = 512, K = 256; for 11-13 M = rows,
- * N = 2; for 14 M = pairs. */
+ * (the maps of cotr_*_attention), 11 match_queries, 12 match_pixels, 13 nearest, 14 mutual (cotr_match_keypoints),
+ * 15 refine_geometry, 16 resize_h, 17 resize_v, 18 refine_step (cotr_refine).  For GEMMs M,N,K are the problem size; for
+ * attention and attention weights M = query rows, N = 512, K = 256; for 11-13 M = rows, N = 2; for 14 M = pairs; for 15
+ * and 18 M = tasks, N = level; for 16-17 M = crops. */
 typedef struct cotr_launch_record {
     int32_t kernel;
     int32_t M, N, K;
@@ -357,6 +390,13 @@ int cotr_test_rowwise(int op, int rows, const float* in_dev, const float* g1_dev
 /* out[(p*nq+i), j] = head-averaged softmax(q k^T) (the maps of cotr_decode_attention); q (npairs*nq,256), k (npairs*512,256),
  * out (npairs,nq,512), all DEVICE.  Path 0 reads k through the attention operand images, path 1 row-major. */
 int cotr_test_attention_weights(int path, const float* q_dev, const float* k_dev, float* out_dev, int nq, int npairs);
+/* The per-task arithmetic of cotr_refine run on the HOST (the same __host__ __device__ functions), n rows:
+ * op 0 crop: in [pos_x, pos_y, scale], in_i [h, w] -> out_i [left, top, size, flag] (size -1: NaN scale; flag 1: NaN or
+ * infinite position, clamped); op 1 query: in [x, y], in_i [px, py, size] -> out fp32 [qx, qy]; op 2 scale_to_loc:
+ * in fp32 [p_x, p_y], in_i [px, py, size] -> out [x, y]; op 3 conclude: in (levels+1) x 2 history, in_i [h_to, w_to]
+ * -> out_i good. */
+int cotr_test_refine_math(int op, int n, int levels, double rel_threshold, const double* in, const int32_t* in_i,
+                          double* out, int32_t* out_i);
 /* bring-up / A-B switches (0 = production): bit 8 (256) disables programmatic dependent launch, bit 9 (512) disables
  * split-K, bits 10-11 move the CTA-count threshold of the 64-wide GEMM tile, bits 14-15 lower the
  * minimum K of split-K (16 >> n chunks of 64).  Schedule: by default a transformer section with >= 2048 rows runs the
