@@ -32,7 +32,7 @@ class TestGemmDesc(ctypes.Structure):
 class TestAttentionDesc(ctypes.Structure):
     _fields_ = [(n, ctypes.c_int32) for n in (
         "path", "nq", "npairs", "operands", "slots", "slot", "ctx_pairs", "pair0", "q_rows", "ldq", "q_col0", "n_tiles",
-        "key_split", "reserved")]
+        "key_split", "maps_rows", "maps_row0", "reserved")]
 
 
 class TestMlpDesc(ctypes.Structure):
@@ -104,10 +104,9 @@ _PROTOTYPES = {
     "cotr_debug_read": (ctypes.c_int64, [ctypes.c_void_p, ctypes.c_char_p, ctypes.c_void_p, ctypes.c_int64]),
     "cotr_set_gemm_path": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_int]),
     "cotr_test_gemm": (ctypes.c_int, [ctypes.POINTER(TestGemmDesc)] + [ctypes.c_void_p] * 12),
-    "cotr_test_attention": (ctypes.c_int, [ctypes.POINTER(TestAttentionDesc)] + [ctypes.c_void_p] * 5),
+    "cotr_test_attention": (ctypes.c_int, [ctypes.POINTER(TestAttentionDesc)] + [ctypes.c_void_p] * 6),
     "cotr_test_mlp": (ctypes.c_int, [ctypes.POINTER(TestMlpDesc)] + [ctypes.c_void_p] * 10),
     "cotr_test_rowwise": (ctypes.c_int, [ctypes.c_int, ctypes.c_int] + [ctypes.c_void_p] * 6),
-    "cotr_test_attention_weights": (ctypes.c_int, [ctypes.c_int] + [ctypes.c_void_p] * 3 + [ctypes.c_int, ctypes.c_int]),
     "cotr_test_refine_math": (ctypes.c_int, [ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_double] + [ctypes.c_void_p] * 4),
     "cotr_debug_set_variant": (None, [ctypes.c_int]),
     "cotr_last_error": (ctypes.c_char_p, []),
@@ -581,25 +580,21 @@ def test_gemm(path, A, w_host, *, bias=None, addmat=None, add_period=1, residual
     return out
 
 
-def test_attention_weights(path, q, k, nq, npairs):
-    """Kernel-level hook: head-averaged softmax(q k^T) -> (npairs, nq, 512) (cotr_test_attention_weights)."""
-    out = torch.zeros((npairs, nq, 512), dtype=torch.float32, device=q.device)
-    check(lib().cotr_test_attention_weights(path, _ptr(q), _ptr(k), _ptr(out), nq, npairs), "cotr_test_attention_weights")
-    return out
-
-
 ATTENTION_OPERANDS = {"rowmajor": 0, "images": 1}
 
 
 def test_attention(path, q, k, v, nq, npairs, *, operands="rowmajor", pair0=0, slot=0, q_col0=0, tiles=None, key_split=0,
-                   out=None):
+                   out=None, maps=None, maps_row0=0):
     """Kernel-level hook: softmax(q k^T) v per head, launched as the model launches it (cotr_test_attention).
 
     q: (rows, ldq) CUDA fp32, the launch reads columns q_col0 .. q_col0+255.  k, v: (ctx_pairs*512, slots*256) CUDA fp32,
     the keys / values of `slots` layers side by side per pair as in a context; the launch reads slot `slot` of pairs
     pair0 .. .  operands: "rowmajor" (fp32 SIMT schedule) or "images" (tensor-core schedule).  tiles: optional (n,3)
     table of (pair, first row, row count) - then nq / npairs are unused.  key_split (path 0): 0 = launch rule, 1 or 2.
-    out: (rows,256) CUDA fp32, rows the launch does not own are returned unchanged (default zeros)."""
+    out: (rows,256) CUDA fp32, rows the launch does not own are returned unchanged (default zeros).
+    maps: optional (maps_rows,512) CUDA fp32, written in place: the head-averaged attention maps of the same operands
+    (path 0 with "images", path 1 with "rowmajor"), local pair p, query i at row maps_row0 + p*nq + i; the other rows
+    are left unchanged."""
     d = TestAttentionDesc()
     d.path, d.nq, d.npairs = path, nq, npairs
     d.operands = ATTENTION_OPERANDS[operands]
@@ -616,8 +611,12 @@ def test_attention(path, q, k, v, nq, npairs, *, operands="rowmajor", pair0=0, s
     if out is None:
         out = torch.zeros((q.shape[0], 256), dtype=torch.float32, device=q.device)
     assert out.is_contiguous() and out.shape == (q.shape[0], 256)
+    if maps is not None:
+        assert maps.is_cuda and maps.dtype == torch.float32 and maps.is_contiguous() and maps.ndim == 2 and maps.shape[1] == 512
+        d.maps_rows, d.maps_row0 = maps.shape[0], maps_row0
     check(lib().cotr_test_attention(ctypes.byref(d), _ptr(q), _ptr(k), _ptr(v), _ptr(out),
-                                    ctypes.c_void_p(tab.ctypes.data) if tab is not None else None), "cotr_test_attention")
+                                    ctypes.c_void_p(tab.ctypes.data) if tab is not None else None,
+                                    _ptr(maps) if maps is not None else None), "cotr_test_attention")
     return out
 
 

@@ -591,17 +591,23 @@ AttnMaps attn_maps(int layer_mask, float* attn_dev, int B, size_t rows) {
     return maps;
 }
 
+// The maps launch over the operands the attention launch `a` reads, local pair p's rows from out + p * out_pair_stride
+AttnWeightsParams attention_weights_params(const AttnParams& a, float* out, size_t out_pair_stride) {
+    AttnWeightsParams p{};
+    p.q = a.q; p.ldq = a.ldq;
+    p.k = a.k; p.ldk = a.ldk;
+    p.kv_img = a.kv_img; p.img_pair_stride = a.img_pair_stride;
+    p.out = out; p.out_pair_stride = out_pair_stride;
+    p.nq = a.nq; p.npairs = a.npairs; p.pair0 = a.pair0;
+    return p;
+}
+
 // The maps of one layer from the operands its attention launch `a` just read (attention_weights.cu); recorded like the
 // attention launch (M = query rows, N = 512 keys, K = 32 x 8 heads).
 int run_attention_weights(const Run& r, const AttnParams& a, const AttnMaps& maps, int layer) {
     float* out = maps.layer(layer);
     if (!out) return 0;
-    AttnWeightsParams p{};
-    p.q = a.q; p.ldq = a.ldq;
-    p.k = a.k; p.ldk = a.ldk;
-    p.kv_img = a.kv_img; p.img_pair_stride = a.img_pair_stride;
-    p.out = out; p.out_pair_stride = maps.pair_stride;
-    p.nq = a.nq; p.npairs = a.npairs; p.pair0 = a.pair0;
+    const AttnWeightsParams p = attention_weights_params(a, out, maps.pair_stride);
     const bool tc = r.m->gemm_path == 0;
     LaunchScope scope(r, tc ? K_ATTN_WEIGHTS_TC : K_ATTN_WEIGHTS_SIMT, a.nq * a.npairs, kTokens, kDModel);
     return tc ? launch_attention_weights_tc(p, r.s) : launch_attention_weights_simt(p, r.s);
@@ -2132,18 +2138,17 @@ std::vector<float> identity(int n) {
     return eye;
 }
 
-// Writes the keys (kv: [rows][256]) or the keys and values (kv: [rows][512] = [K | V]) of every pair into slot `slot`
-// of the `slots` attention operand images per pair at img, by the same epilogue store as the model's projections: a
-// tensor-core GEMM with the identity as its weight.
-int write_operand_images(DevAllocs& mem, CSplit16 kv, int rows, bool values, int slot, int slots, unsigned char* img) {
-    const int n = values ? 2 * kDModel : kDModel;
+// Writes the keys and values (kv: [rows][512] = [K | V]) of every pair into slot `slot` of the `slots` attention
+// operand images per pair at img, by the same epilogue store as the model's projections: a tensor-core GEMM with the
+// identity as its weight.
+int write_operand_images(DevAllocs& mem, CSplit16 kv, int rows, int slot, int slots, unsigned char* img) {
+    const int n = 2 * kDModel;
     const std::vector<float> eye = identity(n);
     void* wtc = nullptr;
     float scale = 1.f;
     if (upload_tc_weight(mem, eye.data(), n, n, &wtc, &scale)) return 1;
     GemmParams p = gemm_base(rows, n, n, kv, n, nullptr, wtc, scale, kNoSplit, n);
-    p.remap = 1; p.blk_map[0] = -1000 - slot; p.n_vt = slots; p.kv_img = img;
-    if (values) p.blk_map[1] = -(slot + 1);
+    p.remap = 1; p.blk_map[0] = -1000 - slot; p.blk_map[1] = -(slot + 1); p.n_vt = slots; p.kv_img = img;
     return launch_gemm_tc(p, 0);
 }
 }  // namespace
@@ -2337,9 +2342,10 @@ int cotr_test_gemm(cotr_test_gemm_desc* d, const float* A_dev, const float* w_ho
 // the chosen schedule, produced by the same epilogue stores as in the model: V transposed by the fp32 SIMT identity
 // GEMM (operands 0), or K and V of the slot as the operand images of one tensor-core identity GEMM over [K | V]
 // (operands 1), the other slots' images left 0xFF (fp16 NaN).  `out` is converted in before the launch, so every row
-// the launch does not own comes back as it was passed.
+// the launch does not own comes back as it was passed.  With `maps` the maps kernel of the path follows, over the
+// AttnParams the attention launch read (as run_attention_weights launches it); it writes fp32 rows straight into maps.
 int cotr_test_attention(const cotr_test_attention_desc* d, const float* q_dev, const float* k_dev, const float* v_dev,
-                        float* out_dev, const int32_t* tiles_host) {
+                        float* out_dev, const int32_t* tiles_host, float* maps_dev) {
     COTR_CHECK(d && q_dev && k_dev && v_dev && out_dev, "cotr_test_attention: null argument");
     COTR_CHECK(d->path == 0 || d->path == 1, "cotr_test_attention: path %d (0 tensor cores, 1 fp32 SIMT)", d->path);
     COTR_CHECK(d->operands == 0 || d->operands == 1, "cotr_test_attention: operands %d (0 row-major, 1 images)", d->operands);
@@ -2372,6 +2378,14 @@ int cotr_test_attention(const cotr_test_attention_desc* d, const float* q_dev, c
                    d->pair0 + d->npairs - 1, d->ctx_pairs);
         COTR_CHECK((int64_t)d->nq * d->npairs <= d->q_rows, "cotr_test_attention: %d x %d rows, q has %d", d->npairs, d->nq, d->q_rows);
     }
+    if (maps_dev) {
+        COTR_CHECK(d->n_tiles == 0, "cotr_test_attention: maps of a tile-table launch (the model asks maps of uniform launches only)");
+        COTR_CHECK(d->path != 0 || d->operands == 1, "cotr_test_attention: tensor-core maps read the keys as operand images (operands 1)");
+        COTR_CHECK(d->path != 1 || d->operands == 0, "cotr_test_attention: fp32 SIMT maps read row-major keys (operands 0)");
+        COTR_CHECK(d->maps_row0 >= 0 && (int64_t)d->maps_row0 + (int64_t)d->npairs * d->nq <= d->maps_rows,
+                   "cotr_test_attention: map rows %d .. %lld do not fit the %d rows of maps", d->maps_row0,
+                   (long long)d->maps_row0 + (int64_t)d->npairs * d->nq - 1, d->maps_rows);
+    }
 
     DevAllocs mem;
     TmpSplit q16, o16, k16, v16, vt16, kv16;
@@ -2392,7 +2406,7 @@ int cotr_test_attention(const cotr_test_attention_desc* d, const float* q_dev, c
                                      kDModel * sizeof(float), kv_rows, cudaMemcpyDeviceToDevice));
         COTR_CHECK_CUDA(cudaMemset(img, 0xFF, img_bytes));
         if (kv16.from_f32(kv, kv_rows * 2 * kDModel) ||
-            write_operand_images(mem, cs(kv16.t), (int)kv_rows, true, d->slot, d->slots, img)) return 1;
+            write_operand_images(mem, cs(kv16.t), (int)kv_rows, d->slot, d->slots, img)) return 1;
         a.kv_img = img + (size_t)d->slot * kHeads * kAttnHeadImgBytes;
         a.img_pair_stride = (size_t)d->slots * kHeads * kAttnHeadImgBytes;
     } else {
@@ -2419,6 +2433,10 @@ int cotr_test_attention(const cotr_test_attention_desc* d, const float* q_dev, c
     int rc;
     if (d->path == 1) rc = launch_attention_simt(a, 0);
     else rc = d->key_split ? launch_attention_tc_split(a, d->key_split, 0) : launch_attention_tc(a, 0);
+    if (!rc && maps_dev) {
+        const AttnWeightsParams w = attention_weights_params(a, maps_dev + (size_t)d->maps_row0 * kTokens, (size_t)d->nq * kTokens);
+        rc = d->path == 0 ? launch_attention_weights_tc(w, 0) : launch_attention_weights_simt(w, 0);
+    }
     if (!rc) rc = launch_split16_to_f32(cs(o16.t), out_dev, (size_t)d->q_rows * kDModel, 0);
     const cudaError_t e = cudaDeviceSynchronize();
     if (rc) return rc;
@@ -2474,38 +2492,6 @@ int cotr_test_rowwise(int op, int rows, const float* in_dev, const float* g1_dev
     const cudaError_t e = cudaDeviceSynchronize();
     if (rc) return rc;
     COTR_CHECK(e == cudaSuccess, "cotr_test_rowwise: kernel failed: %s", cudaGetErrorString(e));
-    return 0;
-}
-
-// q (npairs*nq,256), k (npairs*512,256) fp32 row-major -> out (npairs,nq,512).  Path 0 reads k as the attention operand
-// images, written by the same epilogue store (split16.cuh store16) as in the model, through an identity "GEMM".
-int cotr_test_attention_weights(int path, const float* q_dev, const float* k_dev, float* out_dev, int nq, int npairs) {
-    COTR_CHECK(q_dev && k_dev && out_dev, "cotr_test_attention_weights: null argument");
-    COTR_CHECK(nq >= 1 && npairs >= 1, "cotr_test_attention_weights: nq and npairs must be >= 1");
-    TmpSplit q16, k16;
-    const size_t qn = (size_t)npairs * nq * kDModel, kn = (size_t)npairs * kTokens * kDModel;
-    if (q16.from_f32(q_dev, qn) || k16.from_f32(k_dev, kn)) return 1;
-    AttnWeightsParams a{};
-    a.q = cs(q16.t); a.ldq = kDModel;
-    a.out = out_dev; a.out_pair_stride = (size_t)nq * kTokens;
-    a.nq = nq; a.npairs = npairs; a.pair0 = 0;
-    DevAllocs mem;
-    int rc = 0;
-    if (path == 0) {
-        unsigned char* img = nullptr;
-        const size_t img_bytes = (size_t)npairs * kHeads * kAttnHeadImgBytes;
-        if (mem.alloc((void**)&img, img_bytes)) return 1;
-        COTR_CHECK_CUDA(cudaMemset(img, 0, img_bytes));
-        if (write_operand_images(mem, cs(k16.t), npairs * kTokens, false, 0, 1, img)) return 1;
-        a.kv_img = img; a.img_pair_stride = (size_t)kHeads * kAttnHeadImgBytes;
-        rc = launch_attention_weights_tc(a, 0);
-    } else {
-        a.k = cs(k16.t); a.ldk = kDModel;
-        rc = launch_attention_weights_simt(a, 0);
-    }
-    const cudaError_t e = cudaDeviceSynchronize();
-    if (rc) return rc;
-    COTR_CHECK(e == cudaSuccess, "cotr_test_attention_weights: kernel failed: %s", cudaGetErrorString(e));
     return 0;
 }
 

@@ -364,13 +364,18 @@ typedef struct cotr_test_attention_desc {
     int32_t q_rows, ldq, q_col0;  /* q (q_rows, ldq), the launch reads its columns q_col0 .. q_col0+255; out (q_rows,256) */
     int32_t n_tiles;              /* > 0: tiles_host holds n_tiles (pair, first row, row count) triples (ragged decode) */
     int32_t key_split;            /* path 0: 0 = the launch rule, 1 or 2 = that key split                             */
+    int32_t maps_rows;            /* maps_dev != NULL: maps_dev is (maps_rows, 512) ...                                 */
+    int32_t maps_row0;            /* ... and local pair p, query i of the launch goes to its row maps_row0 + p*nq + i    */
     int32_t reserved;
 } cotr_test_attention_desc;
 /* out[r, h*32+d] = softmax(q k^T) v per head for the rows the launch owns; every other row of out is left as it was
  * passed.  q (q_rows,ldq), k / v (ctx_pairs*512, slots*256), out (q_rows,256): fp32 DEVICE; tiles_host int32 HOST or NULL.
- * Every argument is checked before anything is launched. */
+ * maps_dev (fp32 DEVICE, or NULL: no maps): after the attention launch, the head-averaged attention maps of the same
+ * operands, launched as the model launches them for cotr_*_attention (attention_weights.cu): the tensor-core kernel
+ * (path 0, image operands) or the fp32 SIMT one (path 1, row-major operands); not with a tile table.  Map rows the launch
+ * does not own are left as they were passed.  Every argument is checked before anything is launched. */
 int cotr_test_attention(const cotr_test_attention_desc* d, const float* q_dev, const float* k_dev, const float* v_dev,
-                        float* out_dev, const int32_t* tiles_host);
+                        float* out_dev, const int32_t* tiles_host, float* maps_dev);
 typedef struct cotr_test_mlp_desc {
     int32_t M;                    /* rows of the launch                                                             */
     int32_t rows;                 /* rows of x and out (>= M)                                                        */
@@ -387,9 +392,6 @@ int cotr_test_mlp(const cotr_test_mlp_desc* d, const float* x_dev, const float* 
  * 3 lin_sine query encoding of (rows,2) points in [0,1] (in; g1 .. b2 unused).  in (rows,256), out (rows,256): DEVICE. */
 int cotr_test_rowwise(int op, int rows, const float* in_dev, const float* g1_dev, const float* b1_dev,
                       const float* g2_dev, const float* b2_dev, float* out_dev);
-/* out[(p*nq+i), j] = head-averaged softmax(q k^T) (the maps of cotr_decode_attention); q (npairs*nq,256), k (npairs*512,256),
- * out (npairs,nq,512), all DEVICE.  Path 0 reads k through the attention operand images, path 1 row-major. */
-int cotr_test_attention_weights(int path, const float* q_dev, const float* k_dev, float* out_dev, int nq, int npairs);
 /* The per-task arithmetic of cotr_refine run on the HOST (the same __host__ __device__ functions), n rows:
  * op 0 crop: in [pos_x, pos_y, scale], in_i [h, w] -> out_i [left, top, size, flag] (size -1: NaN scale; flag 1: NaN or
  * infinite position, clamped); op 1 query: in [x, y], in_i [px, py, size] -> out fp32 [qx, qy]; op 2 scale_to_loc:
