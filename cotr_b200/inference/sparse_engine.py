@@ -39,12 +39,16 @@ def _is_fresh(task):
 
 
 def _exact_point(p):
-    """An (x, y) array whose arithmetic in RefinementTask is fp64 arithmetic on its values: float64 and finite, or
-    integers that fp64 holds exactly (Python raises on NaN / inf positions; float32 points compute in float32)."""
+    """An (x, y) array whose arithmetic in RefinementTask is fp64 arithmetic on its values: float64 and finite, float32
+    below 2**24 in magnitude, or integers that fp64 holds exactly (Python raises on NaN / inf positions).
+    float32: `pos - size // 2` and `loc - patch.x` are exact in fp32 where the crop is not clamped (a multiple of ulp(pos)
+    no larger than pos), and an fp64 quotient rounded to fp32 equals the fp32 quotient (53 >= 2 * 24 + 2)."""
     if not (isinstance(p, np.ndarray) and p.shape == (2,)):
         return False
     if p.dtype == np.float64:
         return bool(np.isfinite(p).all())
+    if p.dtype == np.float32:
+        return bool((np.abs(p) < 2.0 ** 24).all())
     return p.dtype.kind in 'iu' and bool((np.abs(p.astype(np.float64)) < 2.0 ** 52).all())
 
 
