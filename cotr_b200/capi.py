@@ -51,7 +51,8 @@ class LaunchRecord(ctypes.Structure):
 
 KERNEL_NAMES = ("gemm_tc", "gemm_simt", "attention_tc", "attention_simt", "layernorm", "maxpool", "query_encode", "stem_canvas", "gemm_mlp",
                 "attention_weights_tc", "attention_weights_simt", "match_queries", "match_pixels", "nearest", "mutual",
-                "refine_geometry", "resize_h", "resize_v", "refine_step")
+                "refine_geometry", "resize_h", "resize_v", "refine_step", "grouped_candidates", "group_tasks", "grouped_geometry",
+                "grouped_step")
 
 # name -> (restype, argtypes); every symbol include/cotr_b200.h declares
 _PROTOTYPES = {
@@ -82,6 +83,10 @@ _PROTOTYPES = {
     "cotr_refine": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p, ctypes.c_int,
                                    ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int64, ctypes.c_double]
                     + [ctypes.c_void_p] * 8),
+    "cotr_refine_grouped": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_void_p, ctypes.c_int,
+                                           ctypes.c_int, ctypes.c_double, ctypes.c_double, ctypes.c_void_p, ctypes.c_int, ctypes.c_int,
+                                           ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int64,
+                                           ctypes.c_double] + [ctypes.c_void_p] * 7),
     "cotr_dense_postprocess": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p]),
     "cotr_flow_tile_merge": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p] + [ctypes.c_int] * 6 +
                              [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p]),
@@ -108,6 +113,7 @@ _PROTOTYPES = {
     "cotr_test_mlp": (ctypes.c_int, [ctypes.POINTER(TestMlpDesc)] + [ctypes.c_void_p] * 10),
     "cotr_test_rowwise": (ctypes.c_int, [ctypes.c_int, ctypes.c_int] + [ctypes.c_void_p] * 6),
     "cotr_test_refine_math": (ctypes.c_int, [ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_double] + [ctypes.c_void_p] * 4),
+    "cotr_test_pilot_boxes": (ctypes.c_int, [ctypes.c_int, ctypes.c_void_p, ctypes.c_int] + [ctypes.c_void_p] * 3),
     "cotr_debug_set_variant": (None, [ctypes.c_int]),
     "cotr_last_error": (ctypes.c_char_p, []),
     "cotr_version": (ctypes.c_char_p, []),
@@ -326,6 +332,22 @@ class NativeModel:
                                 _ptr(loc_from), _ptr(loc_to), _ptr(history), _ptr(rects), _ptr(good), ctypes.byref(walked),
                                 status, self._stream()), "cotr_refine")
         return history, rects, good, walked.value, tuple(status)
+
+    def refine_grouped(self, img_from, img_to, s_from, s_to, zooms, level, ids, batch_size, max_load, max_good, rel_threshold,
+                       loc_from, history, rects, good):
+        """One grouped batch (cotr_refine_grouped).  img_*: uint8 HWC device tensors; ids: the level's open tasks in shuffled
+        order; loc_from (n,2) fp64, history (n,L+1,2) fp64, rects (n,L,6) int32, good (n+1,) int32: device tensors the
+        batches of one walk share -> (squad (n_ids,) int32 numpy, (n_squads, longest, num_steps, stepped, status))."""
+        ids = np.ascontiguousarray(ids, dtype=np.int32)
+        z = np.ascontiguousarray(zooms, dtype=np.float64)
+        squad = np.empty(max(ids.size, 1), dtype=np.int32)
+        result = (ctypes.c_int32 * 5)()
+        check(lib().cotr_refine_grouped(self.handle, _ptr(img_from), img_from.shape[0], img_from.shape[1], _ptr(img_to), img_to.shape[0],
+                                        img_to.shape[1], float(s_from), float(s_to), ctypes.c_void_p(z.ctypes.data), z.size, int(level),
+                                        ctypes.c_void_p(ids.ctypes.data), ids.size, loc_from.shape[0], int(batch_size), int(max_load),
+                                        int(max_good), float(rel_threshold), _ptr(loc_from), _ptr(history), _ptr(rects), _ptr(good),
+                                        ctypes.c_void_p(squad.ctypes.data), result, self._stream()), "cotr_refine_grouped")
+        return squad[:ids.size], tuple(result)
 
     def dense_postprocess(self, pred_dev):
         """(n, 131072, 2) fp32 predictions of the dense grid queries -> (n, 256, 512, 3) [x, y, confidence] (device)."""
@@ -663,3 +685,15 @@ def test_refine_math(op, inputs, ints, levels=1, rel_threshold=0.0):
                                       ctypes.c_void_p(b.ctypes.data), ctypes.c_void_p(out.ctypes.data),
                                       ctypes.c_void_p(out_i.ctypes.data)), "cotr_test_refine_math")
     return out if op in (1, 2) else (out_i if op == 0 else out_i[:, 0])
+
+
+def test_pilot_boxes(pts, geom, device=0):
+    """cotr_test_pilot_boxes: the candidate kernel of cotr_refine_grouped on (n,4) fp64 end points and [h_from, w_from,
+    h_to, w_to, size_from, size_to] -> ((n,8) fp64 pilot boxes, (n,) int32 crop failure codes)."""
+    p = np.ascontiguousarray(pts, dtype=np.float64).reshape(-1, 4)
+    g = np.ascontiguousarray(geom, dtype=np.int32)
+    box = np.zeros((p.shape[0], 8), dtype=np.float64)
+    fail = np.zeros(p.shape[0], dtype=np.int32)
+    check(lib().cotr_test_pilot_boxes(int(device), ctypes.c_void_p(p.ctypes.data), p.shape[0], ctypes.c_void_p(g.ctypes.data),
+                                      ctypes.c_void_p(box.ctypes.data), ctypes.c_void_p(fail.ctypes.data)), "cotr_test_pilot_boxes")
+    return box, fail

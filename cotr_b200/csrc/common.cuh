@@ -385,6 +385,17 @@ int launch_refine_geometry(const RefineLevel& lv, const double* loc_from, const 
 // predictions -> history row l+1; at the last level the good flag and the chunk's good count; NaN flags `status`
 int launch_refine_step(const RefineLevel& lv, const float* pred, const int32_t* rects, double* history, int32_t* good,
                        int32_t* chunk_good, unsigned long long* status, cudaStream_t s);
+// Grouped walk of cotr_refine_grouped: lv.count candidates ids[0 ..) at lv.level.  End points (n,4), pilot boxes (n,8) and
+// the exception code of each candidate's crop (1 NaN, 2 infinite position) for group_tasks_launch.
+int launch_grouped_candidates(const RefineLevel& lv, const int32_t* ids, const double* loc_from, const double* history, double* pts,
+                              double* box, int32_t* fail, cudaStream_t s);
+// squads -> CropSide 2s / 2s+1 of each pilot, every member's rect at this level and its query at row s * longest + rank
+int launch_grouped_geometry(const RefineLevel& lv, const int32_t* ids, const int32_t* squad, const int32_t* rank, int n_squads,
+                            int longest, const double* loc_from, const double* history, CropSide* sides, int32_t* rects,
+                            float* queries, cudaStream_t s);
+// predictions -> history row level+1 of every member; at the last level the good flag and good_count
+int launch_grouped_step(const RefineLevel& lv, const int32_t* ids, const int32_t* squad, const int32_t* rank, int longest,
+                        const float* pred, const int32_t* rects, double* history, int32_t* good, int32_t* good_count, cudaStream_t s);
 
 // Bytes of the pre-tiled fp16 hi/lo image of an [N,K] weight matrix, and the host-side packer (returns acc_scale).
 size_t tc_weight_bytes(int N, int K);

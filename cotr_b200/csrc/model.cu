@@ -107,6 +107,13 @@ struct Workspace {
     CropSide* refine_sides = nullptr;
     unsigned char* refine_tmp = nullptr;
     unsigned long long* refine_counts = nullptr;
+    // grouped walk (cotr_refine_grouped; canvases, crop table and horizontal-pass bytes are the walk's above): one batch's
+    // candidate end points and pilot boxes, its table [n_squads | squad | fail | rank], and the (squads, longest)
+    // queries and predictions
+    int64_t cap_grouped_ids = 0, cap_grouped_rows = 0;
+    double *grouped_pts = nullptr, *grouped_box = nullptr;
+    int32_t* grouped_tab = nullptr;
+    float *grouped_q = nullptr, *grouped_pred = nullptr;
 };
 
 // A host table that reaches the device with one asynchronous copy per call, staged through pinned memory.  `copied` is
@@ -188,6 +195,7 @@ struct cotr_model {
     cotr::PinnedTable<int> pair_tab;     // cotr_encode_context_pairs: the caller's (B,2) image table
     cotr::PinnedTable<int4> tile_tab;    // cotr_decode_ragged: the attention tile tables of all chunks of a call (AttnParams::tiles)
     cotr::PinnedTable<int4> match_tab;   // cotr_match_keypoints: the match tiles and pair table of a call (MatchPlan::tab)
+    cotr::PinnedTable<int32_t> grouped_ids;   // cotr_refine_grouped: the batch's permuted candidate task ids
     cotr::Preprocessor* pre = nullptr;         // device-side crop / resize / normalise (cotr_preprocess)
     cotr::FlowMerger* merger = nullptr;        // device-side tail of the dense first guess (cotr_flow_tile_merge)
     bool prof_on = false;
@@ -373,7 +381,8 @@ struct Run {
 
 enum KernelId { K_GEMM_TC = 0, K_GEMM_SIMT = 1, K_ATTN_TC = 2, K_ATTN_SIMT = 3, K_LAYERNORM = 4, K_MAXPOOL = 5, K_QENC = 6, K_STEM_CANVAS = 7,
                 K_GEMM_MLP = 8, K_ATTN_WEIGHTS_TC = 9, K_ATTN_WEIGHTS_SIMT = 10, K_MATCH_QUERIES = 11, K_MATCH_PIXELS = 12,
-                K_NEAREST = 13, K_MUTUAL = 14, K_REFINE_GEOMETRY = 15, K_RESIZE_H = 16, K_RESIZE_V = 17, K_REFINE_STEP = 18 };
+                K_NEAREST = 13, K_MUTUAL = 14, K_REFINE_GEOMETRY = 15, K_RESIZE_H = 16, K_RESIZE_V = 17, K_REFINE_STEP = 18,
+                K_GROUPED_CANDIDATES = 19, K_GROUP_TASKS = 20, K_GROUPED_GEOMETRY = 21, K_GROUPED_STEP = 22 };
 
 // Counts the launch and, when the profiler is on, brackets it with two events on the launching stream.
 struct LaunchScope {
@@ -681,6 +690,12 @@ std::vector<WsBuf> refine_ws_bufs(Workspace& w, int tasks, size_t tmp, int64_t c
             ws_raw(&w.refine_counts, 1 + ((size_t)chunks + 1) / 2)};
 }
 
+// Grouped walk: `ids` candidates of one batch, `rows` query rows (squads x longest).
+std::vector<WsBuf> grouped_ws_bufs(Workspace& w, int64_t ids, int64_t rows) {
+    return {ws_raw(&w.grouped_pts, (size_t)ids * 4), ws_raw(&w.grouped_box, (size_t)ids * 8), ws_raw(&w.grouped_tab, 1 + (size_t)ids * 3),
+            ws_raw(&w.grouped_q, (size_t)rows * 2), ws_raw(&w.grouped_pred, (size_t)rows * 2)};
+}
+
 void ws_release(const std::vector<WsBuf>& bufs) {
     for (const WsBuf& b : bufs) {
         if (b.split) ws_free(b.split);
@@ -829,6 +844,20 @@ int ensure_refine_ws(cotr_model* m, int tasks, size_t tmp, int64_t chunks) {
     ws_release(refine_ws_bufs(w, 0, 0, 0));
     if (ws_allocate(refine_ws_bufs(w, tasks, tmp, chunks))) return 1;
     w.cap_refine_tasks = tasks; w.cap_refine_tmp = tmp; w.cap_refine_chunks = chunks;
+    return 0;
+}
+
+// The same for the grouped walk's own buffers.
+int ensure_grouped_ws(cotr_model* m, int64_t ids, int64_t rows) {
+    Workspace& w = m->ws;
+    if (ids <= w.cap_grouped_ids && rows <= w.cap_grouped_rows) return 0;
+    ids = std::max(ids, w.cap_grouped_ids);
+    rows = std::max(rows, w.cap_grouped_rows);
+    COTR_CHECK_CUDA(cudaDeviceSynchronize());
+    w.cap_grouped_ids = 0; w.cap_grouped_rows = 0;    // as in ensure_encode_ws
+    ws_release(grouped_ws_bufs(w, 0, 0));
+    if (ws_allocate(grouped_ws_bufs(w, ids, rows))) return 1;
+    w.cap_grouped_ids = ids; w.cap_grouped_rows = rows;
     return 0;
 }
 
@@ -1500,6 +1529,7 @@ void cotr_destroy(cotr_model* m) {
     ws_release(decode_ws_bufs(w, 0));
     ws_release(match_ws_bufs(w, 0));
     ws_release(refine_ws_bufs(w, 0, 0, 0));
+    ws_release(grouped_ws_bufs(w, 0, 0));
     for (float** b : {&w.img_stage, &w.q_stage, &w.pred_stage}) ws_free_f32(b);
     if (m->host_stream) cudaStreamDestroy(m->host_stream);
     for (auto& kv : m->graphs) cudaGraphExecDestroy(kv.second);
@@ -1827,6 +1857,96 @@ int refine_walk_impl(cotr_model* m, const uint8_t* const* images, const int32_t*
     return 0;
 }
 
+// One grouped batch of cotr_refine_grouped, arguments checked; fs / ts are the level's two crop sides.  The candidates'
+// end points and pilot boxes, and the squads, are made on the device; one small copy brings back the squad table, the
+// candidates' crop failures and, while the max_corrs stop can fall, the good count.  Then the batch either ends there
+// (a pilot whose crop raises in Python), or only writes its rects (the max_corrs stop: the squads are submitted, not
+// stepped), or enqueues its geometry, canvases, forward and step without another wait.
+int refine_grouped_impl(cotr_model* m, const uint8_t* img_from, int h_from, int w_from, const uint8_t* img_to, int h_to, int w_to,
+                        int fs, int ts, int level, int L, const int32_t* ids_host, int n_ids, int n_tasks, int batch_size,
+                        int max_load, int64_t max_good, double rel, const double* loc_from, double* history, int32_t* rects,
+                        int32_t* good, int32_t* squad_host, int32_t* result, cudaStream_t s) {
+    for (int k = 0; k < 5; ++k) result[k] = 0;
+    m->launches = 0;
+    if (n_ids == 0) return 0;
+    if (!m->pre) m->pre = preprocessor_create();
+    RefineLevel lv = RefineLevel();
+    lv.task0 = 0; lv.count = n_ids; lv.level = level; lv.levels = L; lv.chunk = 0;
+    lv.h_from = h_from; lv.w_from = w_from; lv.h_to = h_to; lv.w_to = w_to;
+    lv.thr = refine_threshold(rel, h_to, w_to);
+    lv.from.img = img_from; lv.from.img_w = w_from;
+    lv.to.img = img_to; lv.to.img_w = w_to;
+    if (preprocess_coeffs(m->pre, fs, &lv.from) || preprocess_coeffs(m->pre, ts, &lv.to)) return 1;
+    // every buffer at its largest for this batch before the first launch: growing one later would drop the squad table
+    const int64_t max_squads = std::min(batch_size, n_ids);
+    const int64_t max_rows = max_squads * std::min<int64_t>((int64_t)max_load + 1, n_ids);
+    if (ensure_refine_ws(m, (int)max_squads, (size_t)max_squads * (fs + ts) * 256 * 3, 0)) return 1;
+    if (ensure_grouped_ws(m, n_ids, max_rows)) return 1;
+    if (m->grouped_ids.upload(ids_host, (size_t)n_ids, s)) return 1;
+    Workspace& w = m->ws;
+    const int32_t* ids = m->grouped_ids.dev;
+    int32_t* n_squads_dev = w.grouped_tab;
+    int32_t* squad = w.grouped_tab + 1;
+    int32_t* fail = squad + n_ids;
+    int32_t* rank = fail + n_ids;
+
+    Run r{m, s};
+    {
+        LaunchScope scope(r, K_GROUPED_CANDIDATES, n_ids, level, 0);
+        if (launch_grouped_candidates(lv, ids, loc_from, history, w.grouped_pts, w.grouped_box, fail, s)) return 1;
+    }
+    {
+        LaunchScope scope(r, K_GROUP_TASKS, n_ids, level, 0);
+        if (group_tasks_launch(w.grouped_pts, w.grouped_box, n_ids, batch_size, max_load, squad, rank, n_squads_dev, s)) return 1;
+    }
+    std::vector<int32_t> tab(1 + 2 * (size_t)n_ids);
+    int32_t good_count = 0;
+    const bool read_good = max_good > 0 && max_good <= n_tasks;     // otherwise the count cannot decide the stop
+    COTR_CHECK_CUDA(cudaMemcpyAsync(tab.data(), w.grouped_tab, tab.size() * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
+    if (read_good) COTR_CHECK_CUDA(cudaMemcpyAsync(&good_count, good + n_tasks, sizeof(int32_t), cudaMemcpyDeviceToHost, s));
+    COTR_CHECK_CUDA(cudaStreamSynchronize(s));
+    const int n_squads = tab[0];
+    std::vector<int> members((size_t)n_squads, 0);
+    int num_steps = 0, status = 0;
+    for (int i = 0; i < n_ids; ++i) {
+        const int sq = tab[1 + i];
+        squad_host[i] = sq;
+        if (sq < 0) continue;
+        // a squad's pilot precedes its members in list order, and pilots come in squad order: the first failing pilot
+        // met here is the one at which the host loop raises
+        if (members[sq] == 0 && status == 0) status = tab[1 + n_ids + i];
+        ++members[sq];
+        ++num_steps;
+    }
+    const int longest = n_squads ? *std::max_element(members.begin(), members.end()) : 0;
+    result[0] = n_squads; result[1] = longest; result[2] = num_steps; result[4] = status;
+    if (status != 0 || n_squads == 0) return 0;
+    const bool step = !(max_good <= 0 || (read_good && good_count >= max_good));
+    COTR_CHECK_CUDA(cudaMemsetAsync(w.grouped_q, 0, (size_t)n_squads * longest * 2 * sizeof(float), s));    // padding rows
+    {
+        LaunchScope scope(r, K_GROUPED_GEOMETRY, n_ids, level, 0);
+        if (launch_grouped_geometry(lv, ids, squad, rank, n_squads, longest, loc_from, history, w.refine_sides, rects, w.grouped_q, s)) return 1;
+    }
+    if (!step) return 0;
+    {
+        LaunchScope scope(r, K_RESIZE_H, 2 * n_squads, 0, 0);
+        if (launch_resize_h(w.refine_sides, 2 * n_squads, std::max(fs, ts), w.refine_tmp, s)) return 1;
+    }
+    {
+        LaunchScope scope(r, K_RESIZE_V, 2 * n_squads, 0, 0);
+        if (launch_resize_v(w.refine_sides, 2 * n_squads, w.refine_tmp, w.refine_canvas, s)) return 1;
+    }
+    const int launches = m->launches;     // forward_eager counts its own launches from 0
+    if (forward_eager(m, w.refine_canvas, w.grouped_q, n_squads, longest, w.grouped_pred, s)) return 1;
+    {
+        LaunchScope scope(r, K_GROUPED_STEP, n_ids, level, 0);
+        if (launch_grouped_step(lv, ids, squad, rank, longest, w.grouped_pred, rects, history, good, good + n_tasks, s)) return 1;
+    }
+    m->launches += launches;
+    result[3] = 1;
+    return 0;
+}
+
 }  // namespace
 
 int cotr_forward(cotr_model* m, const float* img_dev, const float* queries_dev, int B, int Q, float* pred_dev, void* cuda_stream) {
@@ -1922,6 +2042,76 @@ int cotr_refine(cotr_model* m, const uint8_t* const* images_host, const int32_t*
     CallOrder order(m, s);
     return refine_walk_impl(m, images_host, hw_host, groups_host, n_groups, sizes, n_zoom, batch, wave, max_good, rel_threshold,
                             loc_from_dev, loc_to_dev, history_dev, rects_dev, good_dev, walked_host, status_host, s);
+}
+
+int cotr_refine_grouped(cotr_model* m, const uint8_t* img_from_dev, int h_from, int w_from, const uint8_t* img_to_dev, int h_to,
+                        int w_to, double s_from, double s_to, const double* zoom_host, int n_zoom, int level, const int32_t* ids_host,
+                        int n_ids, int n_tasks, int batch_size, int max_load, int64_t max_good, double rel_threshold,
+                        const double* loc_from_dev, double* history_dev, int32_t* rects_dev, int32_t* good_dev, int32_t* squad_host,
+                        int32_t* result_host, void* cuda_stream) {
+    const char* fn = "cotr_refine_grouped";
+    COTR_CHECK(m != nullptr, "%s: null model", fn);
+    COTR_CHECK(result_host && zoom_host, "%s: null result_host or zoom_host", fn);
+    COTR_CHECK(img_from_dev && img_to_dev, "%s: null image", fn);
+    COTR_CHECK(h_from >= 2 && w_from >= 2 && h_to >= 2 && w_to >= 2, "%s: images %d x %d and %d x %d", fn, h_from, w_from, h_to, w_to);
+    COTR_CHECK(n_zoom >= 1 && n_zoom <= 7, "%s: %d zoom levels (1 .. 7: conclude() sums the history sequentially)", fn, n_zoom);
+    COTR_CHECK(level >= 0 && level < n_zoom, "%s: level %d of %d", fn, level, n_zoom);
+    COTR_CHECK(batch_size >= 1 && max_load >= 0, "%s: batch_size (%d) must be >= 1 and max_load (%d) >= 0", fn, batch_size, max_load);
+    COTR_CHECK(n_tasks >= 1 && n_ids >= 0 && n_ids <= n_tasks, "%s: %d candidates of %d tasks", fn, n_ids, n_tasks);
+    COTR_CHECK(n_ids == 0 || (ids_host && squad_host), "%s: null ids_host or squad_host", fn);
+    std::vector<char> seen((size_t)n_tasks, 0);
+    for (int i = 0; i < n_ids; ++i) {
+        const int32_t t = ids_host[i];
+        COTR_CHECK(t >= 0 && t < n_tasks && !seen[t], "%s: candidate %d is task %d (outside [0, %d) or repeated)", fn, i, t, n_tasks);
+        seen[t] = 1;
+    }
+    int sizes[2];
+    for (int side = 0; side < 2; ++side) {
+        const int h = side ? h_to : h_from, w = side ? w_to : w_from;
+        sizes[side] = refine_crop_size(h, w, (side ? s_to : s_from) * zoom_host[level]);
+        COTR_CHECK(sizes[side] >= 2 && sizes[side] <= h && sizes[side] <= w, "%s: level %d: %s crop side %d in a %d x %d image", fn, level,
+                   side ? "to" : "from", sizes[side], h, w);
+    }
+    COTR_CHECK(loc_from_dev && history_dev && rects_dev && good_dev, "%s: null device buffer", fn);
+    COTR_CHECK(((uintptr_t)loc_from_dev & 7) == 0 && ((uintptr_t)history_dev & 7) == 0, "%s: loc_from_dev or history_dev is not 8-byte aligned", fn);
+    COTR_CHECK(((uintptr_t)rects_dev & 3) == 0 && ((uintptr_t)good_dev & 3) == 0, "%s: rects_dev or good_dev is not 4-byte aligned", fn);
+    COTR_CHECK_CUDA(cudaSetDevice(m->device));
+    cudaStream_t s = (cudaStream_t)cuda_stream;
+    CallOrder order(m, s);
+    return refine_grouped_impl(m, img_from_dev, h_from, w_from, img_to_dev, h_to, w_to, sizes[0], sizes[1], level, n_zoom, ids_host, n_ids,
+                               n_tasks, batch_size, max_load, max_good, rel_threshold, loc_from_dev, history_dev, rects_dev, good_dev,
+                               squad_host, result_host, s);
+}
+
+int cotr_test_pilot_boxes(int device, const double* pts_host, int n, const int32_t* geom_host, double* box_host, int32_t* fail_host) {
+    const char* fn = "cotr_test_pilot_boxes";
+    COTR_CHECK(n >= 1 && pts_host && geom_host && box_host && fail_host, "%s: bad arguments", fn);
+    const int32_t* g = geom_host;
+    COTR_CHECK(g[4] >= 2 && g[4] <= g[0] && g[4] <= g[1] && g[5] >= 2 && g[5] <= g[2] && g[5] <= g[3], "%s: bad geometry", fn);
+    COTR_CHECK_CUDA(cudaSetDevice(device));
+    // the launch reads candidate i as task i at level 0 of a one-level walk: loc_from (n,2), history (n,2,2) row 0
+    std::vector<double> lf((size_t)n * 2), hist((size_t)n * 4, 0.0);
+    std::vector<int32_t> ids((size_t)n);
+    for (int i = 0; i < n; ++i) {
+        lf[2 * i] = pts_host[4 * i]; lf[2 * i + 1] = pts_host[4 * i + 1];
+        hist[4 * i] = pts_host[4 * i + 2]; hist[4 * i + 1] = pts_host[4 * i + 3];
+        ids[i] = i;
+    }
+    DevAllocs d;
+    void *lf_dev, *hist_dev, *ids_dev, *pts_dev, *box_dev, *fail_dev;
+    if (d.upload(&lf_dev, lf.data(), lf.size() * sizeof(double)) || d.upload(&hist_dev, hist.data(), hist.size() * sizeof(double)) ||
+        d.upload(&ids_dev, ids.data(), ids.size() * sizeof(int32_t)) || d.alloc(&pts_dev, (size_t)n * 4 * sizeof(double)) ||
+        d.alloc(&box_dev, (size_t)n * 8 * sizeof(double)) || d.alloc(&fail_dev, (size_t)n * sizeof(int32_t)))
+        return 1;
+    RefineLevel lv = RefineLevel();
+    lv.count = n; lv.level = 0; lv.levels = 1;
+    lv.h_from = g[0]; lv.w_from = g[1]; lv.h_to = g[2]; lv.w_to = g[3];
+    lv.from.size = g[4]; lv.to.size = g[5];
+    if (launch_grouped_candidates(lv, (const int32_t*)ids_dev, (const double*)lf_dev, (const double*)hist_dev, (double*)pts_dev,
+                                  (double*)box_dev, (int32_t*)fail_dev, 0)) return 1;
+    COTR_CHECK_CUDA(cudaMemcpy(box_host, box_dev, (size_t)n * 8 * sizeof(double), cudaMemcpyDeviceToHost));
+    COTR_CHECK_CUDA(cudaMemcpy(fail_host, fail_dev, (size_t)n * sizeof(int32_t), cudaMemcpyDeviceToHost));
+    return 0;
 }
 
 int cotr_dense_postprocess(cotr_model* m, const float* pred_dev, int n, float* out_dev, void* cuda_stream) {

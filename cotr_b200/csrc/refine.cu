@@ -167,6 +167,126 @@ __global__ void __launch_bounds__(128) refine_step_kernel(RefineLevel lv, const 
     }
 }
 
+// ---- grouped walk (cotr_refine_grouped): FasterSparseEngine's squads at one level ----------------------------------
+
+// Corner of a candidate's pilot box as FasterSparseEngine._pilot_boxes computes it: np.trunc(pos - size // 2) cast to
+// int64, max(., 0), shifted back inside.  numpy's cast gives INT64_MIN on x86-64 for NaN, +-inf and |x| >= 2**63, which
+// max(., 0) turns into 0; for those positions get_patch_centered_at's int() raises (NaN, inf) or is exact (huge finite
+// values land at limit - size), so only the box follows numpy here.  A NaN or infinite position only matters in a box
+// when its task becomes a pilot, and then the host loop raises at the pilot's crop anyway.
+__device__ inline int box_corner(double pos, int size, int limit) {
+    const double d = d_sub(pos, (double)(size / 2));
+    if (!(fabs(trunc(d)) < 9223372036854775808.0)) return 0;
+    int flag = 0;
+    return patch_corner(pos, size, limit, &flag);
+}
+
+// Python's order of failure at a pilot's crops: get_patch_centered_at takes top (y) before left (x), and the "from"
+// crop before the "to" crop.  1 = int(NaN) (ValueError), 2 = int(+-inf) (OverflowError), 0 = none.
+__device__ inline int crop_failure(double x, double y, int prev) {
+    if (prev) return prev;
+    if (y != y) return 1;
+    if (y == INFINITY || y == -INFINITY) return 2;
+    if (x != x) return 1;
+    if (x == INFINITY || x == -INFINITY) return 2;
+    return 0;
+}
+
+// Per candidate i (task ids[i], list order): its end points [loc_from, location at this level], the central-half boxes
+// of the crops it would impose as a pilot (form_squad's safe_box: centre +- size / 4, all exact in fp64) and the
+// exception its crop would raise.
+__global__ void __launch_bounds__(128) grouped_candidates_kernel(RefineLevel lv, const int32_t* __restrict__ ids,
+                                                                 const double* __restrict__ loc_from, const double* __restrict__ history,
+                                                                 double* __restrict__ pts, double* __restrict__ box,
+                                                                 int32_t* __restrict__ fail) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= lv.count) return;
+    const size_t t = (size_t)ids[i];
+    const double* lf = loc_from + 2 * t;
+    const double* lt = history + (t * (lv.levels + 1) + lv.level) * 2;
+    double* p = pts + (size_t)i * 4;
+    p[0] = lf[0]; p[1] = lf[1]; p[2] = lt[0]; p[3] = lt[1];
+    const int fs = lv.from.size, ts = lv.to.size;
+    const int corner[4] = {box_corner(lf[0], fs, lv.w_from), box_corner(lf[1], fs, lv.h_from),
+                           box_corner(lt[0], ts, lv.w_to), box_corner(lt[1], ts, lv.h_to)};
+    double* b = box + (size_t)i * 8;
+#pragma unroll
+    for (int side = 0; side < 2; ++side) {
+        const double size = side ? ts : fs;
+        const double half = d_mul(d_div(size, 2.0), 0.5);
+        const double cx = d_add((double)corner[2 * side], d_div(size, 2.0)), cy = d_add((double)corner[2 * side + 1], d_div(size, 2.0));
+        b[4 * side + 0] = d_sub(cx, half);
+        b[4 * side + 1] = d_add(cx, half);
+        b[4 * side + 2] = d_sub(cy, half);
+        b[4 * side + 3] = d_add(cy, half);
+    }
+    fail[i] = crop_failure(lt[0], lt[1], crop_failure(lf[0], lf[1], 0));
+}
+
+// One CTA per squad: the pilot's crops (get_patch_centered_at) become CropSide 2s / 2s+1 and the rect of this level of
+// every member (the pilot's two patches, as get_task_pilot submits them), and each member's canvas query is its own
+// loc_from in the pilot's "from" patch, at row s * longest + rank (pilot first, then the members in list order).
+__global__ void __launch_bounds__(256) grouped_geometry_kernel(RefineLevel lv, const int32_t* __restrict__ ids,
+                                                               const int32_t* __restrict__ squad, const int32_t* __restrict__ rank,
+                                                               int n_squads, int longest, const double* __restrict__ loc_from,
+                                                               const double* __restrict__ history, CropSide* __restrict__ sides,
+                                                               int32_t* __restrict__ rects, float* __restrict__ queries) {
+    __shared__ int s_rect[4];
+    const int s = blockIdx.x;
+    const int fs = lv.from.size, ts = lv.to.size;
+    for (int i = threadIdx.x; i < lv.count; i += blockDim.x) {
+        if (squad[i] != s || rank[i] != 0) continue;
+        const size_t t = (size_t)ids[i];
+        const double* lf = loc_from + 2 * t;
+        const double* lt = history + (t * (lv.levels + 1) + lv.level) * 2;
+        int flag = 0;       // a non-finite pilot position was reported by grouped_candidates_kernel; the call stops first
+        CropSide a = lv.from, b = lv.to;
+        a.x = patch_corner(lf[0], fs, lv.w_from, &flag);
+        a.y = patch_corner(lf[1], fs, lv.h_from, &flag);
+        b.x = patch_corner(lt[0], ts, lv.w_to, &flag);
+        b.y = patch_corner(lt[1], ts, lv.h_to, &flag);
+        a.tmp_offset = (size_t)s * fs * 256 * 3;
+        b.tmp_offset = (size_t)n_squads * fs * 256 * 3 + (size_t)s * ts * 256 * 3;
+        sides[2 * s] = a;
+        sides[2 * s + 1] = b;
+        s_rect[0] = a.x; s_rect[1] = a.y; s_rect[2] = b.x; s_rect[3] = b.y;
+    }
+    __syncthreads();
+    const int ax = s_rect[0], ay = s_rect[1], bx = s_rect[2], by = s_rect[3];
+    for (int i = threadIdx.x; i < lv.count; i += blockDim.x) {
+        if (squad[i] != s) continue;
+        const size_t t = (size_t)ids[i];
+        int32_t* r = rects + (t * lv.levels + lv.level) * 6;
+        r[0] = ax; r[1] = ay; r[2] = fs; r[3] = bx; r[4] = by; r[5] = ts;
+        const float2 q = query_in(loc_from[2 * t], loc_from[2 * t + 1], ax, ay, fs);
+        float* out = queries + ((size_t)s * longest + rank[i]) * 2;
+        out[0] = q.x;
+        out[1] = q.y;
+    }
+}
+
+// RefinementTask.step for every member: scale_to_loc with its pilot's "to" patch into history row level + 1; at the
+// last level conclude(), the good flag and good[n] += 1.
+__global__ void __launch_bounds__(128) grouped_step_kernel(RefineLevel lv, const int32_t* __restrict__ ids, const int32_t* __restrict__ squad,
+                                                           const int32_t* __restrict__ rank, int longest, const float* __restrict__ pred,
+                                                           const int32_t* __restrict__ rects, double* __restrict__ history,
+                                                           int32_t* __restrict__ good, int32_t* __restrict__ good_count) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= lv.count || squad[i] < 0) return;
+    const size_t t = (size_t)ids[i];
+    const float* p = pred + ((size_t)squad[i] * longest + rank[i]) * 2;
+    const int32_t* r = rects + (t * lv.levels + lv.level) * 6;
+    const double2 loc = scale_to_loc(p[0], p[1], r[3], r[4], r[5]);
+    double* h = history + t * (lv.levels + 1) * 2;
+    h[2 * (lv.level + 1)] = loc.x;
+    h[2 * (lv.level + 1) + 1] = loc.y;
+    if (lv.level == lv.levels - 1) {
+        const bool g = conclude_good(h, lv.levels + 1, lv.thr);
+        good[t] = g ? 1 : 0;
+        if (g) atomicAdd(good_count, 1);
+    }
+}
+
 constexpr int kRefineThreads = 128;
 
 }  // namespace
@@ -198,6 +318,30 @@ int launch_refine_step(const RefineLevel& lv, const float* pred, const int32_t* 
                        int32_t* chunk_good, unsigned long long* status, cudaStream_t s) {
     refine_step_kernel<<<(lv.count + kRefineThreads - 1) / kRefineThreads, kRefineThreads, 0, s>>>(lv, pred, rects, history, good,
                                                                                                   chunk_good, status);
+    COTR_CHECK_CUDA(cudaGetLastError());
+    return 0;
+}
+
+int launch_grouped_candidates(const RefineLevel& lv, const int32_t* ids, const double* loc_from, const double* history, double* pts,
+                              double* box, int32_t* fail, cudaStream_t s) {
+    grouped_candidates_kernel<<<(lv.count + kRefineThreads - 1) / kRefineThreads, kRefineThreads, 0, s>>>(lv, ids, loc_from, history,
+                                                                                                         pts, box, fail);
+    COTR_CHECK_CUDA(cudaGetLastError());
+    return 0;
+}
+
+int launch_grouped_geometry(const RefineLevel& lv, const int32_t* ids, const int32_t* squad, const int32_t* rank, int n_squads,
+                            int longest, const double* loc_from, const double* history, CropSide* sides, int32_t* rects,
+                            float* queries, cudaStream_t s) {
+    grouped_geometry_kernel<<<n_squads, 256, 0, s>>>(lv, ids, squad, rank, n_squads, longest, loc_from, history, sides, rects, queries);
+    COTR_CHECK_CUDA(cudaGetLastError());
+    return 0;
+}
+
+int launch_grouped_step(const RefineLevel& lv, const int32_t* ids, const int32_t* squad, const int32_t* rank, int longest,
+                        const float* pred, const int32_t* rects, double* history, int32_t* good, int32_t* good_count, cudaStream_t s) {
+    grouped_step_kernel<<<(lv.count + kRefineThreads - 1) / kRefineThreads, kRefineThreads, 0, s>>>(lv, ids, squad, rank, longest, pred,
+                                                                                                   rects, history, good, good_count);
     COTR_CHECK_CUDA(cudaGetLastError());
     return 0;
 }

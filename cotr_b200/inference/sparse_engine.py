@@ -52,6 +52,38 @@ def _exact_point(p):
     return p.dtype.kind in 'iu' and bool((np.abs(p.astype(np.float64)) < 2.0 ** 52).all())
 
 
+def _submit_rect(t, rect):
+    """RefinementTask._submit of a job whose crops are `rect` [x_from, y_from, size_from, x_to, y_to, size_to] (its own or
+    its pilot's), with the device-pixel paths' 'img' key."""
+    x0, y0, s0, x1, y1, s1 = (int(v) for v in rect)
+    (h_f, w_f), (h_t, w_t) = t.image_from.shape[:2], t.image_to.shape[:2]
+    t.cur_job = {'patch_from': ImagePatch(None, x0, y0, s0, s0, w_f, h_f), 'patch_to': ImagePatch(None, x1, y1, s1, s1, w_t, h_t),
+                 'loc_from': t.loc_from, 'loc_to': t.cur_loc_to, 'img': None}
+    t.job_history.append((s0, s0, s1, s1))
+
+
+def _replay_level(t, rect, loc, good):
+    """What a device walk did to task `t` at its current level, as the host loop leaves it: submit with `rect`, then
+    RefinementTask.step to `loc` (fp64 (2,)) with converge_iters 1, and next_zoom; `good` decides the last level."""
+    _submit_rect(t, rect)
+    last = t.cur_zoom_idx == len(t.zoom_ins) - 1
+    loc = loc.copy()
+    t.total_iter += 1
+    t.loc_to_at_zoom.append(loc)
+    if last:
+        t.cur_iter += 1
+    t.all_loc_to_dict[t.cur_zoom] = np.array(t.loc_to_at_zoom).copy()
+    t.loc_history.append(loc)
+    t.best_loc_to = loc
+    t.cur_loc_to = loc
+    if last:
+        t.status = 'finished'
+        t.result = 'good' if good else 'bad'
+    t.cur_zoom_idx += 1
+    t.cur_iter = 0
+    t.loc_to_at_zoom = []
+
+
 def _rect_of(task):
     pf, pt = task.cur_job['patch_from'], task.cur_job['patch_to']
     assert pf.w == pf.h and pt.w == pt.h
@@ -272,9 +304,12 @@ class SparseEngine():
                     num_g += t.result == 'good'
 
     def _device_walk_fits(self, tasks):
-        """The walk's conditions: device pixels, fresh tasks with converge_iters 1, one (s_from, s_to) and one zoom
+        return hasattr(self.model, 'refine_walk') and self._walk_fits(tasks)
+
+    def _walk_fits(self, tasks):
+        """The device walks' conditions: device pixels, fresh tasks with converge_iters 1, one (s_from, s_to) and one zoom
         schedule of <= 7 levels, and every crop at least 2 pixels wide (anything else raises in the host loop too)."""
-        if not tasks or not hasattr(self.model, 'refine_walk') or not self._use_device_pixels(tasks):
+        if not tasks or not self._use_device_pixels(tasks):
             return False
         first = tasks[0]
         zooms = list(first.zoom_ins)
@@ -316,30 +351,9 @@ class SparseEngine():
             self.total_tasks += (min(walked + batch, n) - walked) * (level + 1)
             raise ValueError('NaN in prediction' if code == 1 else 'non-finite position in the zoom-in walk')
         print(f'{num_g} / {max_corrs} | {num_f} / {n}')
-        (h_f, w_f), (h_t, w_t) = first.image_from.shape[:2], first.image_to.shape[:2]
         for i in range(walked):
-            t = tasks[i]
             for l in range(L):
-                x0, y0, s0, x1, y1, s1 = (int(v) for v in rects[i, l])
-                t.cur_job = {'patch_from': ImagePatch(None, x0, y0, s0, s0, w_f, h_f), 'patch_to': ImagePatch(None, x1, y1, s1, s1, w_t, h_t),
-                             'loc_from': t.loc_from, 'loc_to': t.cur_loc_to, 'img': None}
-                t.job_history.append((s0, s0, s1, s1))
-                # RefinementTask.step + next_zoom with one iteration per level
-                loc = history[i, l + 1].copy()
-                t.total_iter += 1
-                t.loc_to_at_zoom.append(loc)
-                if l == L - 1:
-                    t.cur_iter += 1
-                t.all_loc_to_dict[t.cur_zoom] = np.array(t.loc_to_at_zoom).copy()
-                t.loc_history.append(loc)
-                t.best_loc_to = loc
-                t.cur_loc_to = loc
-                if l == L - 1:
-                    t.status = 'finished'
-                    t.result = 'good' if good[i] else 'bad'
-                t.cur_zoom_idx += 1
-                t.cur_iter = 0
-                t.loc_to_at_zoom = []
+                _replay_level(tasks[i], rects[i, l], history[i, l + 1], l == L - 1 and bool(good[i]))
         # the host loop forms (submits) the next batch before it tests max_corrs and stops
         for t in tasks[walked:walked + batch]:
             t.get_task_fast()
@@ -540,6 +554,76 @@ class FasterSparseEngine(SparseEngine):
             img_batch = torch.stack(imgs)
         return task_ref, img_batch, torch.cat(queries)
 
+    def _grouped_walk_fits(self, tasks, zoom_ins):
+        """The device walk of the grouped levels applies: the single-query walk's conditions, device grouping, no attention
+        hooks (the host loop fires them per batch), pairwise distinct zoom values (with a repeated one `_is_open` matches
+        tasks of two levels and all_loc_to_dict merges them), and float64 end points in get_tasks_map (float32 points
+        on both ends would be compared in float32 there)."""
+        if not (self.device_walk and self.device_grouping and hasattr(self.model, 'refine_grouped_batch')):
+            return False
+        if not (isinstance(self.batch_size, int) and self.batch_size >= 1 and isinstance(self.max_load, int) and self.max_load >= 0):
+            return False
+        if self.model.attention_hooked() or not self._walk_fits(tasks):
+            return False
+        zooms = [float(z) for z in tasks[0].zoom_ins]
+        if len(set(zooms)) != len(zooms) or [float(z) for z in zoom_ins] != zooms:
+            return False
+        return np.result_type(*{a.dtype for t in tasks for a in (t.loc_from, t.cur_loc_to)}) == np.float64
+
+    def _grouped_walk(self, tasks, zoom_ins, max_corrs):
+        """The `for zm in zoom_ins` loop of cotr_corr_multiscale with one COTR.refine_grouped_batch call per grouped batch:
+        the same np.random.permutation calls, printed lines and task attributes as the host loop.  The host keeps each
+        level's open tasks (those stepped at the level before and not yet taken) in index order."""
+        first = tasks[0]
+        n, L = len(tasks), len(first.zoom_ins)
+        dev = next(self.model.parameters()).device
+        image_from, image_to = self._device_image(first.image_from), self._device_image(first.image_to)
+        history = torch.zeros((n, L + 1, 2), dtype=torch.float64)
+        history[:, 0] = torch.from_numpy(np.array([t.cur_loc_to for t in tasks], dtype=np.float64))
+        walk = {'loc_from': torch.from_numpy(np.array([t.loc_from for t in tasks], dtype=np.float64)).to(dev),
+                'history': history.to(dev), 'rects': torch.zeros((n, L, 6), dtype=torch.int32, device=dev),
+                'good': torch.zeros(n + 1, dtype=torch.int32, device=dev)}
+        # num_g >= max_corrs, with num_g counting the good tasks on the device (NaN max_corrs never stops)
+        max_good = math.ceil(max_corrs) if max_corrs <= n else n + 1
+        steps = np.zeros(n, dtype=np.int64)             # levels each task was stepped at
+        submitted = np.zeros(n, dtype=bool)             # formed into a squad at the max_corrs stop, never stepped
+        open_ids = np.arange(n)
+        for l, zm in enumerate(zoom_ins):
+            print(f'======= Zoom: {zm} ======')
+            stepped = []
+            while True:
+                ids = np.take(open_ids, np.random.permutation(open_ids.shape[0]), axis=0)
+                squad, (n_squads, longest, num_steps, ran, status) = self.model.refine_grouped_batch(
+                    image_from, image_to, first.s_from, first.s_to, [float(z) for z in first.zoom_ins], l, ids, self.batch_size,
+                    self.max_load, max_good, refinement_task.THRESHOLD_PIXELS_RELATIVE, walk)
+                if status == 1:
+                    raise ValueError('cannot convert float NaN to integer')
+                if status == 2:
+                    raise OverflowError('cannot convert float infinity to integer')
+                if n_squads == 0:
+                    break
+                taken = ids[squad >= 0]
+                open_ids = np.sort(ids[squad < 0])
+                if not ran:
+                    submitted[taken] = True
+                    break
+                steps[taken] += 1
+                stepped.append(taken)
+                print(f'solved {num_steps} sub-tasks in one invocation with {n_squads} image pairs')
+                if num_steps <= self.batch_size:
+                    break
+            open_ids = np.sort(np.concatenate(stepped)) if stepped else np.zeros(0, dtype=np.int64)
+        history = walk['history'].cpu().numpy()
+        rects = walk['rects'].cpu().numpy()
+        good = walk['good'].cpu().numpy()
+        for i in np.flatnonzero((steps > 0) | submitted):
+            t = tasks[i]
+            for l in range(steps[i]):
+                _replay_level(t, rects[i, l], history[i, l + 1], l == L - 1 and bool(good[i]))
+            if submitted[i]:
+                _submit_rect(t, rects[i, steps[i]])
+                t.submitted = True
+
     def cotr_corr_multiscale(self, img_a, img_b, zoom_ins=[1.0], converge_iters=1, max_corrs=1000, queries_a=None,
                              return_idx=False, force=False, return_tasks_only=False, areas=None):
         img_a = img_a.copy()
@@ -547,22 +631,26 @@ class FasterSparseEngine(SparseEngine):
         if queries_a is not None:
             queries_a = queries_a.copy()
         tasks = self.gen_tasks(img_a, img_b, zoom_ins, converge_iters, max_corrs, queries_a, force, areas)
-        for zm in zoom_ins:
-            print(f'======= Zoom: {zm} ======')
-            while True:
-                num_g = self.num_good_tasks(tasks)
-                task_ref, img_batch, query_batch = self.form_grouped_batch(zm, tasks)
-                if len(task_ref) == 0 or num_g >= max_corrs:
-                    break
-                out = self.infer_batch_grouped(img_batch, query_batch)
-                num_steps = 0
-                for i, squad in enumerate(task_ref):
-                    for j, t in enumerate(squad):
-                        t.step(out[i, j])
-                        num_steps += 1
-                print(f'solved {num_steps} sub-tasks in one invocation with {img_batch.shape[0]} image pairs')
-                if num_steps <= self.batch_size:     # grouping no longer pays at this level (:398-399)
-                    break
+        if self._grouped_walk_fits(tasks, zoom_ins):
+            self._grouped_walk(tasks, zoom_ins, max_corrs)
+            zm = zoom_ins[-1]
+        else:
+            for zm in zoom_ins:
+                print(f'======= Zoom: {zm} ======')
+                while True:
+                    num_g = self.num_good_tasks(tasks)
+                    task_ref, img_batch, query_batch = self.form_grouped_batch(zm, tasks)
+                    if len(task_ref) == 0 or num_g >= max_corrs:
+                        break
+                    out = self.infer_batch_grouped(img_batch, query_batch)
+                    num_steps = 0
+                    for i, squad in enumerate(task_ref):
+                        for j, t in enumerate(squad):
+                            t.step(out[i, j])
+                            num_steps += 1
+                    print(f'solved {num_steps} sub-tasks in one invocation with {img_batch.shape[0]} image pairs')
+                    if num_steps <= self.batch_size:     # grouping no longer pays at this level (:398-399)
+                        break
         # one-query-per-context fallback, only for tasks sitting at the LAST zoom value (:401-411)
         self._single_query_loop(tasks, max_corrs, zm)
         if self.rescue_stranded:

@@ -366,6 +366,24 @@ class COTR(nn.Module):
                                                                     rel_threshold, lf, lt)
         return history.cpu().numpy(), rects.cpu().numpy(), good.cpu().numpy(), walked, status
 
+    def attention_hooked(self):
+        """True when a forward hook sits on an attention module: the forward then fires it, the device walks cannot."""
+        enc, dec = self._attention_modules()
+        return bool(self._hooked(enc) or self._hooked(dec))
+
+    @torch.no_grad()
+    def refine_grouped_batch(self, img_from, img_to, s_from, s_to, zooms, level, ids, batch_size, max_load, max_good,
+                             rel_threshold, walk):
+        """One grouped batch of FasterSparseEngine's zoom-in on the device (cotr_refine_grouped).  img_*: uint8 HWC CUDA
+        tensors; ids: the open tasks of `level` in shuffled order; walk: the device tensors the batches of one engine call
+        share, {'loc_from': (n,2) fp64, 'history': (n,L+1,2) fp64 with row 0 the first guesses, 'rects': (n,L,6) int32,
+        'good': (n+1,) int32 zeroed}.  Returns (squad (n_ids,) int32: the squad of each candidate or -1,
+        (n_squads, longest, num_steps, stepped, status)); status 1 / 2: a pilot's crop raises (NaN / infinite position)."""
+        if self.attention_hooked():
+            raise RuntimeError("refine_grouped_batch does not fire attention hooks: remove them or use the host loop")
+        return self.native().refine_grouped(img_from, img_to, s_from, s_to, zooms, level, ids, batch_size, max_load, max_good,
+                                            rel_threshold, walk['loc_from'], walk['history'], walk['rects'], walk['good'])
+
     @torch.no_grad()
     def dense_postprocess(self, pred):
         """Device-side tail of the dense pass (inference_helper.py:131-145): (n,131072,2) predictions of the canvas grid

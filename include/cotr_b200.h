@@ -212,6 +212,35 @@ int cotr_refine(cotr_model* m, const uint8_t* const* images_host, const int32_t*
                 double* history_dev, int32_t* rects_dev, int32_t* good_dev, int64_t* walked_host, int32_t* status_host,
                 void* cuda_stream);
 
+/* One grouped batch of FasterSparseEngine's zoom-in with converge_iters = 1 (COTR/inference/sparse_engine.py:339-369
+ * form_grouped_batch and form_squad, :383-399 the batch loop of cotr_corr_multiscale, refinement_task.py:71-85
+ * get_task_pilot) on the device, bit for bit.  The caller keeps the open tasks of each level and draws the permutation:
+ * ids_host holds the n_ids open tasks of level `level` in the engine's shuffled order (distinct, in [0, n_tasks)).
+ *   1. Candidate i gets its end points [loc_from, history row `level`] and the central-half boxes of the crops it would
+ *      impose as a pilot (get_patch_centered_at, with _pilot_boxes' int64 cast); squads form as in cotr_group_tasks.
+ *   2. One small copy brings back the squads: squad_host[i] = squad of candidate i or -1.  result_host: 5 int32
+ *      [n_squads, longest squad, members (num_steps), stepped, status].  status 1 / 2: the crop of a pilot raises in
+ *      Python (int() of a NaN / infinite position: ValueError / OverflowError); the call then stops there.
+ *   3. The squads are submitted: row `level` of rects_dev of every member is its pilot's crop pair.  When max_good <= 0,
+ *      or good_dev[n_tasks] >= max_good (read in the same copy, only when max_good <= n_tasks), the batch stops here
+ *      (stepped 0): the engine's max_corrs stop, which comes after the batch is formed.
+ *   4. Otherwise (stepped 1) the pilots' canvases, the forward of cotr_forward at (n_squads, longest) with each member's
+ *      query (its own loc_from in the pilot's "from" patch; rows pilot first, then the members in list order; zero
+ *      padded) and, per member, scale_to_loc with the pilot's "to" patch into history row level + 1; at the last level
+ *      conclude() into good_dev[t] and the count good_dev[n_tasks].  No wait after step 2.
+ *   img_*_dev: uint8 HWC (3 channels) DEVICE images; crop sides min(h, w) * clip(s * zoom_host[level], 0, 1) rounded down
+ *   to even must be >= 2.  loc_from_dev: n_tasks x 2 fp64; history_dev: n_tasks x (L+1) x 2 fp64 (row 0 = first guesses,
+ *   filled by the caller); rects_dev: n_tasks x L x 6 int32 as in cotr_refine; good_dev: n_tasks + 1 int32 (the caller
+ *   zeroes the count before the first batch).  L = n_zoom, 1 .. 7.  Every argument is checked before anything is
+ *   enqueued; the candidate tables, queries and predictions are model-owned and grow on demand, and the canvases are
+ *   cotr_refine's.  Launches: grouped_candidates, group_tasks, then grouped_geometry, and when stepped resize_h,
+ *   resize_v, the forward, grouped_step. */
+int cotr_refine_grouped(cotr_model* m, const uint8_t* img_from_dev, int h_from, int w_from, const uint8_t* img_to_dev, int h_to,
+                        int w_to, double s_from, double s_to, const double* zoom_host, int n_zoom, int level, const int32_t* ids_host,
+                        int n_ids, int n_tasks, int batch_size, int max_load, int64_t max_good, double rel_threshold,
+                        const double* loc_from_dev, double* history_dev, int32_t* rects_dev, int32_t* good_dev, int32_t* squad_host,
+                        int32_t* result_host, void* cuda_stream);
+
 /* Device-side post-processing of the dense first guess (COTR/inference/inference_helper.py:131-145, the host work of
  * cotr_patch_flow_exhaustive after the 131 072-query forward): pred_dev holds n x (256*512) x 2 fp32 predictions for the
  * grid queries (j/512, i/256) in row-major (i, j) order; out_dev receives n x 256 x 512 x 3 fp32
@@ -295,9 +324,10 @@ int cotr_last_launch_count(const cotr_model* m);
  * kernel ids: 0 gemm_tc (wgmma), 1 gemm_simt, 2 attention_tc, 3 attention_simt, 4 layernorm, 5 maxpool,
  * 6 query_encode, 7 stem_canvas, 8 gemm_mlp (fused feed-forward block), 9 attention_weights_tc, 10 attention_weights_simt
  * (the maps of cotr_*_attention), 11 match_queries, 12 match_pixels, 13 nearest, 14 mutual (cotr_match_keypoints),
- * 15 refine_geometry, 16 resize_h, 17 resize_v, 18 refine_step (cotr_refine).  For GEMMs M,N,K are the problem size; for
+ * 15 refine_geometry, 16 resize_h, 17 resize_v, 18 refine_step (cotr_refine), 19 grouped_candidates, 20 group_tasks,
+ * 21 grouped_geometry, 22 grouped_step (cotr_refine_grouped, with 16-17).  For GEMMs M,N,K are the problem size; for
  * attention and attention weights M = query rows, N = 512, K = 256; for 11-13 M = rows, N = 2; for 14 M = pairs; for 15
- * and 18 M = tasks, N = level; for 16-17 M = crops. */
+ * and 18 M = tasks, N = level; for 16-17 M = crops; for 19-22 M = candidates, N = level. */
 typedef struct cotr_launch_record {
     int32_t kernel;
     int32_t M, N, K;
@@ -399,6 +429,10 @@ int cotr_test_rowwise(int op, int rows, const float* in_dev, const float* g1_dev
  * -> out_i good. */
 int cotr_test_refine_math(int op, int n, int levels, double rel_threshold, const double* in, const int32_t* in_i,
                           double* out, int32_t* out_i);
+/* The candidate kernel of cotr_refine_grouped on n candidates: pts_host n x 4 fp64 [x_from, y_from, x_to, y_to] (HOST),
+ * geom_host [h_from, w_from, h_to, w_to, size_from, size_to] -> box_host n x 8 fp64 pilot boxes, fail_host n int32
+ * (0, 1 NaN, 2 infinite position: the exception the pilot's crop raises in Python).  `device` is the CUDA device index. */
+int cotr_test_pilot_boxes(int device, const double* pts_host, int n, const int32_t* geom_host, double* box_host, int32_t* fail_host);
 /* bring-up / A-B switches (0 = production): bit 8 (256) disables programmatic dependent launch, bit 9 (512) disables
  * split-K, bits 10-11 move the CTA-count threshold of the 64-wide GEMM tile, bits 14-15 lower the
  * minimum K of split-K (16 >> n chunks of 64).  Schedule: by default a transformer section with >= 2048 rows runs the
