@@ -51,8 +51,7 @@ class LaunchRecord(ctypes.Structure):
 
 KERNEL_NAMES = ("gemm_tc", "gemm_simt", "attention_tc", "attention_simt", "layernorm", "maxpool", "query_encode", "stem_canvas", "gemm_mlp",
                 "attention_weights_tc", "attention_weights_simt", "match_queries", "match_pixels", "nearest", "mutual",
-                "refine_geometry", "resize_h", "resize_v", "refine_step", "grouped_candidates", "group_tasks", "grouped_geometry",
-                "grouped_step")
+                "refine_geometry", "resize_h", "resize_v", "refine_step", "grouped_candidates", "group_tasks")
 
 # name -> (restype, argtypes); every symbol include/cotr_b200.h declares
 _PROTOTYPES = {

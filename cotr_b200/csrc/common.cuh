@@ -367,35 +367,32 @@ int preprocess_coeffs(Preprocessor* p, int size, CropSide* side);
 int launch_resize_h(const CropSide* sides, int n_sides, int max_size, unsigned char* tmp, cudaStream_t s);
 int launch_resize_v(const CropSide* sides, int n_sides, const unsigned char* tmp, float* canvas, cudaStream_t s);
 
-// Zoom-in walk of cotr_refine (refine.cu).  One chunk level: the crops of `count` tasks from task0 at one zoom level.
+// Zoom-in walks of cotr_refine and cotr_refine_grouped (refine.cu).  One level: the crops of `count` entries at one zoom
+// level, entry i being task task0 + ids[i].
 struct RefineLevel {
     int task0, count;
     int level, levels;          // level l of L
-    int chunk;                  // chunk index in the call's walk order
-    CropSide from, to;          // everything but x, y and tmp_offset (set per task by the geometry kernel)
+    int chunk;                  // chunk index in cotr_refine's walk order (0 in cotr_refine_grouped)
+    CropSide from, to;          // everything but x, y and tmp_offset (set per squad by the geometry kernel)
     int h_from, w_from, h_to, w_to;
     double thr;                 // rel_threshold * max(h_to, w_to, 3): conclude()'s bound on the history's std
 };
 // get_patch_centered_at's crop side for an h x w image at `scale` (-1 for a NaN scale, where Python raises)
 int refine_crop_size(int h, int w, double scale);
 double refine_threshold(double rel, int h_to, int w_to);
-// task i's crops -> CropSide 2i / 2i+1, rects[(t * L + l) * 6 ..], fp32 canvas query; non-finite positions flag `status`
-int launch_refine_geometry(const RefineLevel& lv, const double* loc_from, const double* history, CropSide* sides,
-                           int32_t* rects, float* queries, unsigned long long* status, cudaStream_t s);
-// predictions -> history row l+1; at the last level the good flag and the chunk's good count; NaN flags `status`
-int launch_refine_step(const RefineLevel& lv, const float* pred, const int32_t* rects, double* history, int32_t* good,
-                       int32_t* chunk_good, unsigned long long* status, cudaStream_t s);
+// squads -> CropSide 2s / 2s+1 of each pilot, every member's rect at this level and its query at row s * longest + rank;
+// non-finite pilot positions flag `status`
+int launch_refine_geometry(const RefineLevel& lv, const int32_t* ids, const int32_t* squad, const int32_t* rank, int n_squads,
+                           int longest, const double* loc_from, const double* history, CropSide* sides, int32_t* rects,
+                           float* queries, unsigned long long* status, cudaStream_t s);
+// predictions -> history row level+1 of every member; at the last level the good flag and good_count; NaN flags `status`
+int launch_refine_step(const RefineLevel& lv, const int32_t* ids, const int32_t* squad, const int32_t* rank, int longest,
+                       const float* pred, const int32_t* rects, double* history, int32_t* good, int32_t* good_count,
+                       unsigned long long* status, cudaStream_t s);
 // Grouped walk of cotr_refine_grouped: lv.count candidates ids[0 ..) at lv.level.  End points (n,4), pilot boxes (n,8) and
 // the exception code of each candidate's crop (1 NaN, 2 infinite position) for group_tasks_launch.
 int launch_grouped_candidates(const RefineLevel& lv, const int32_t* ids, const double* loc_from, const double* history, double* pts,
                               double* box, int32_t* fail, cudaStream_t s);
-// squads -> CropSide 2s / 2s+1 of each pilot, every member's rect at this level and its query at row s * longest + rank
-int launch_grouped_geometry(const RefineLevel& lv, const int32_t* ids, const int32_t* squad, const int32_t* rank, int n_squads,
-                            int longest, const double* loc_from, const double* history, CropSide* sides, int32_t* rects,
-                            float* queries, cudaStream_t s);
-// predictions -> history row level+1 of every member; at the last level the good flag and good_count
-int launch_grouped_step(const RefineLevel& lv, const int32_t* ids, const int32_t* squad, const int32_t* rank, int longest,
-                        const float* pred, const int32_t* rects, double* history, int32_t* good, int32_t* good_count, cudaStream_t s);
 
 // Bytes of the pre-tiled fp16 hi/lo image of an [N,K] weight matrix, and the host-side packer (returns acc_scale).
 size_t tc_weight_bytes(int N, int K);

@@ -76,6 +76,13 @@ struct DecLayer {
 
 const Split16 kNoSplit = {nullptr, nullptr};
 
+// Sizes of the zoom-in walks' workspace: crop pairs (squads) of one level, its query rows, the entries of one level
+// launch, horizontal-pass bytes and cotr_refine's chunks.
+struct RefineCaps {
+    int64_t squads = 0, rows = 0, ids = 0, chunks = 0;
+    size_t tmp = 0;
+};
+
 struct Workspace {
     int cap_pairs = 0;
     int cap_rows = 0;
@@ -98,22 +105,18 @@ struct Workspace {
     // keypoint matching (cotr_match_keypoints): the (rows,2) canvas queries and predictions of one call
     int64_t cap_match_rows = 0;
     float *match_q = nullptr, *match_pred = nullptr;
-    // zoom-in walk (cotr_refine): one chunk's canvases, crop table, horizontal-pass bytes, queries and predictions, and
-    // the call's status word followed by its per-chunk good counts
-    int cap_refine_tasks = 0;
-    size_t cap_refine_tmp = 0;
-    int64_t cap_refine_chunks = 0;
+    // zoom-in walks (cotr_refine, cotr_refine_grouped): one level's canvases, crop table, horizontal-pass bytes and
+    // (squads, longest) queries and predictions; the status word followed by cotr_refine's per-chunk good counts; the
+    // squad tables of cotr_refine's squads of one (0 .. ids-1 and zeros); cotr_refine_grouped's candidate end points and
+    // pilot boxes and its table [n_squads | squad | fail | rank]
+    RefineCaps cap_refine;
     float *refine_canvas = nullptr, *refine_q = nullptr, *refine_pred = nullptr;
     CropSide* refine_sides = nullptr;
     unsigned char* refine_tmp = nullptr;
     unsigned long long* refine_counts = nullptr;
-    // grouped walk (cotr_refine_grouped; canvases, crop table and horizontal-pass bytes are the walk's above): one batch's
-    // candidate end points and pilot boxes, its table [n_squads | squad | fail | rank], and the (squads, longest)
-    // queries and predictions
-    int64_t cap_grouped_ids = 0, cap_grouped_rows = 0;
+    int32_t *refine_iota = nullptr, *refine_zeros = nullptr;
     double *grouped_pts = nullptr, *grouped_box = nullptr;
     int32_t* grouped_tab = nullptr;
-    float *grouped_q = nullptr, *grouped_pred = nullptr;
 };
 
 // A host table that reaches the device with one asynchronous copy per call, staged through pinned memory.  `copied` is
@@ -382,7 +385,7 @@ struct Run {
 enum KernelId { K_GEMM_TC = 0, K_GEMM_SIMT = 1, K_ATTN_TC = 2, K_ATTN_SIMT = 3, K_LAYERNORM = 4, K_MAXPOOL = 5, K_QENC = 6, K_STEM_CANVAS = 7,
                 K_GEMM_MLP = 8, K_ATTN_WEIGHTS_TC = 9, K_ATTN_WEIGHTS_SIMT = 10, K_MATCH_QUERIES = 11, K_MATCH_PIXELS = 12,
                 K_NEAREST = 13, K_MUTUAL = 14, K_REFINE_GEOMETRY = 15, K_RESIZE_H = 16, K_RESIZE_V = 17, K_REFINE_STEP = 18,
-                K_GROUPED_CANDIDATES = 19, K_GROUP_TASKS = 20, K_GROUPED_GEOMETRY = 21, K_GROUPED_STEP = 22 };
+                K_GROUPED_CANDIDATES = 19, K_GROUP_TASKS = 20 };
 
 // Counts the launch and, when the profiler is on, brackets it with two events on the launching stream.
 struct LaunchScope {
@@ -683,17 +686,13 @@ std::vector<WsBuf> match_ws_bufs(Workspace& w, int64_t rows) {
     return {ws_raw(&w.match_q, (size_t)rows * 2), ws_raw(&w.match_pred, (size_t)rows * 2)};
 }
 
-// Zoom-in walk: chunks of `tasks` tasks, `tmp` horizontal-pass bytes, `chunks` per-chunk counters (2 per u64) + status.
-std::vector<WsBuf> refine_ws_bufs(Workspace& w, int tasks, size_t tmp, int64_t chunks) {
-    return {ws_raw(&w.refine_canvas, (size_t)tasks * 3 * COTR_CANVAS_H * COTR_CANVAS_W), ws_raw(&w.refine_q, (size_t)tasks * 2),
-            ws_raw(&w.refine_pred, (size_t)tasks * 2), ws_raw(&w.refine_sides, (size_t)tasks * 2), ws_raw(&w.refine_tmp, tmp),
-            ws_raw(&w.refine_counts, 1 + ((size_t)chunks + 1) / 2)};
-}
-
-// Grouped walk: `ids` candidates of one batch, `rows` query rows (squads x longest).
-std::vector<WsBuf> grouped_ws_bufs(Workspace& w, int64_t ids, int64_t rows) {
-    return {ws_raw(&w.grouped_pts, (size_t)ids * 4), ws_raw(&w.grouped_box, (size_t)ids * 8), ws_raw(&w.grouped_tab, 1 + (size_t)ids * 3),
-            ws_raw(&w.grouped_q, (size_t)rows * 2), ws_raw(&w.grouped_pred, (size_t)rows * 2)};
+// Zoom-in walks: the per-chunk counters are 2 per u64, after the status word.
+std::vector<WsBuf> refine_ws_bufs(Workspace& w, const RefineCaps& c) {
+    return {ws_raw(&w.refine_canvas, (size_t)c.squads * 3 * COTR_CANVAS_H * COTR_CANVAS_W), ws_raw(&w.refine_sides, (size_t)c.squads * 2),
+            ws_raw(&w.refine_tmp, c.tmp), ws_raw(&w.refine_q, (size_t)c.rows * 2), ws_raw(&w.refine_pred, (size_t)c.rows * 2),
+            ws_raw(&w.refine_counts, 1 + ((size_t)c.chunks + 1) / 2), ws_raw(&w.refine_iota, (size_t)c.ids),
+            ws_raw(&w.refine_zeros, (size_t)c.ids), ws_raw(&w.grouped_pts, (size_t)c.ids * 4), ws_raw(&w.grouped_box, (size_t)c.ids * 8),
+            ws_raw(&w.grouped_tab, 1 + (size_t)c.ids * 3)};
 }
 
 void ws_release(const std::vector<WsBuf>& bufs) {
@@ -833,31 +832,26 @@ int ensure_match_ws(cotr_model* m, int64_t rows) {
 }
 
 // Never captured in a graph either; every capacity only grows.
-int ensure_refine_ws(cotr_model* m, int tasks, size_t tmp, int64_t chunks) {
+int ensure_refine_ws(cotr_model* m, RefineCaps need) {
     Workspace& w = m->ws;
-    if (tasks <= w.cap_refine_tasks && tmp <= w.cap_refine_tmp && chunks <= w.cap_refine_chunks) return 0;
-    tasks = std::max(tasks, w.cap_refine_tasks);
-    tmp = std::max(tmp, w.cap_refine_tmp);
-    chunks = std::max(chunks, w.cap_refine_chunks);
+    RefineCaps& cap = w.cap_refine;
+    if (need.squads <= cap.squads && need.rows <= cap.rows && need.ids <= cap.ids && need.chunks <= cap.chunks && need.tmp <= cap.tmp)
+        return 0;
+    need.squads = std::max(need.squads, cap.squads);
+    need.rows = std::max(need.rows, cap.rows);
+    need.ids = std::max(need.ids, cap.ids);
+    need.chunks = std::max(need.chunks, cap.chunks);
+    need.tmp = std::max(need.tmp, cap.tmp);
     COTR_CHECK_CUDA(cudaDeviceSynchronize());
-    w.cap_refine_tasks = 0; w.cap_refine_tmp = 0; w.cap_refine_chunks = 0;    // as in ensure_encode_ws
-    ws_release(refine_ws_bufs(w, 0, 0, 0));
-    if (ws_allocate(refine_ws_bufs(w, tasks, tmp, chunks))) return 1;
-    w.cap_refine_tasks = tasks; w.cap_refine_tmp = tmp; w.cap_refine_chunks = chunks;
-    return 0;
-}
-
-// The same for the grouped walk's own buffers.
-int ensure_grouped_ws(cotr_model* m, int64_t ids, int64_t rows) {
-    Workspace& w = m->ws;
-    if (ids <= w.cap_grouped_ids && rows <= w.cap_grouped_rows) return 0;
-    ids = std::max(ids, w.cap_grouped_ids);
-    rows = std::max(rows, w.cap_grouped_rows);
-    COTR_CHECK_CUDA(cudaDeviceSynchronize());
-    w.cap_grouped_ids = 0; w.cap_grouped_rows = 0;    // as in ensure_encode_ws
-    ws_release(grouped_ws_bufs(w, 0, 0));
-    if (ws_allocate(grouped_ws_bufs(w, ids, rows))) return 1;
-    w.cap_grouped_ids = ids; w.cap_grouped_rows = rows;
+    cap = RefineCaps();       // as in ensure_encode_ws
+    ws_release(refine_ws_bufs(w, cap));
+    if (ws_allocate(refine_ws_bufs(w, need))) return 1;
+    std::vector<int32_t> iota((size_t)need.ids);
+    for (size_t i = 0; i < iota.size(); ++i) iota[i] = (int32_t)i;
+    COTR_CHECK_CUDA(cudaMemcpy(w.refine_iota, iota.data(), iota.size() * sizeof(int32_t), cudaMemcpyHostToDevice));
+    COTR_CHECK_CUDA(cudaMemset(w.refine_zeros, 0, iota.size() * sizeof(int32_t)));
+    COTR_CHECK_CUDA(cudaDeviceSynchronize());     // both tables written before a call on a non-blocking stream reads them
+    cap = need;
     return 0;
 }
 
@@ -1528,8 +1522,7 @@ void cotr_destroy(cotr_model* m) {
     ws_release(encode_ws_bufs(w, 0));
     ws_release(decode_ws_bufs(w, 0));
     ws_release(match_ws_bufs(w, 0));
-    ws_release(refine_ws_bufs(w, 0, 0, 0));
-    ws_release(grouped_ws_bufs(w, 0, 0));
+    ws_release(refine_ws_bufs(w, RefineCaps()));
     for (float** b : {&w.img_stage, &w.q_stage, &w.pred_stage}) ws_free_f32(b);
     if (m->host_stream) cudaStreamDestroy(m->host_stream);
     for (auto& kv : m->graphs) cudaGraphExecDestroy(kv.second);
@@ -1737,6 +1730,62 @@ int forward_staged(cotr_model* m, int B, int Q, cudaStream_t s) {
     return forward_eager(m, w.img_stage, w.q_stage, B, Q, w.pred_stage, s);
 }
 
+// get_patch_centered_at's two crop sides of one level into sizes[0] ("from") and sizes[1] ("to"), each checked to be at
+// least 2 and to fit its image; `where` opens the error message.
+int refine_crop_sides(const char* where, int level, double zoom, int h_from, int w_from, double s_from, int h_to, int w_to, double s_to,
+                      int* sizes) {
+    for (int side = 0; side < 2; ++side) {
+        const int h = side ? h_to : h_from, w = side ? w_to : w_from;
+        sizes[side] = refine_crop_size(h, w, (side ? s_to : s_from) * zoom);
+        COTR_CHECK(sizes[side] >= 2 && sizes[side] <= h && sizes[side] <= w, "%s: level %d: %s crop side %d in a %d x %d image", where,
+                   level, side ? "to" : "from", sizes[side], h, w);
+    }
+    return 0;
+}
+
+// The crop template of level `level` of L from one image to another: everything of a RefineLevel but its entries (task0,
+// count, chunk), with the Pillow coefficient tables of both crop sides (uploaded once per side length).
+int refine_level_template(cotr_model* m, const uint8_t* img_from, int h_from, int w_from, const uint8_t* img_to, int h_to, int w_to,
+                          int fs, int ts, int level, int L, double rel, RefineLevel* lv) {
+    if (!m->pre) m->pre = preprocessor_create();
+    *lv = RefineLevel();
+    lv->level = level; lv->levels = L;
+    lv->h_from = h_from; lv->w_from = w_from; lv->h_to = h_to; lv->w_to = w_to;
+    lv->thr = refine_threshold(rel, h_to, w_to);
+    lv->from.img = img_from; lv->from.img_w = w_from;
+    lv->to.img = img_to; lv->to.img_w = w_to;
+    return preprocess_coeffs(m->pre, fs, &lv->from) || preprocess_coeffs(m->pre, ts, &lv->to);
+}
+
+// One level of a zoom-in walk (refine.cu's entries, squads and tables), enqueued without a wait: the pilots' crops, rects
+// and queries, then, when `step`, their canvases, the forward at (n_squads, longest) and every member's step, with the
+// good count going to *good_count.  Adds its launches to m->launches.
+int refine_level(cotr_model* m, const RefineLevel& lv, const int32_t* ids, const int32_t* squad, const int32_t* rank, int n_squads,
+                 int longest, bool step, const double* loc_from, double* history, int32_t* rects, int32_t* good, int32_t* good_count,
+                 cudaStream_t s) {
+    Workspace& w = m->ws;
+    Run r{m, s};
+    {
+        LaunchScope scope(r, K_REFINE_GEOMETRY, lv.count, lv.level, 0);
+        if (launch_refine_geometry(lv, ids, squad, rank, n_squads, longest, loc_from, history, w.refine_sides, rects, w.refine_q,
+                                   w.refine_counts, s)) return 1;
+    }
+    if (!step) return 0;
+    {
+        LaunchScope scope(r, K_RESIZE_H, 2 * n_squads, 0, 0);
+        if (launch_resize_h(w.refine_sides, 2 * n_squads, std::max(lv.from.size, lv.to.size), w.refine_tmp, s)) return 1;
+    }
+    {
+        LaunchScope scope(r, K_RESIZE_V, 2 * n_squads, 0, 0);
+        if (launch_resize_v(w.refine_sides, 2 * n_squads, w.refine_tmp, w.refine_canvas, s)) return 1;
+    }
+    const int launches = m->launches;     // forward_eager counts its own launches from 0
+    if (forward_eager(m, w.refine_canvas, w.refine_q, n_squads, longest, w.refine_pred, s)) return 1;
+    m->launches += launches;
+    LaunchScope scope(r, K_REFINE_STEP, lv.count, lv.level, 0);
+    return launch_refine_step(lv, ids, squad, rank, longest, w.refine_pred, rects, history, good, good_count, w.refine_counts, s);
+}
+
 // The zoom-in walk of cotr_refine, arguments checked.  sizes: n_groups x L x 2 crop sides.  The host loop's batches
 // fall on the chunks: its first `batch` open tasks are the first chunk not yet finished, and after one step each of them
 // is open again one level deeper, so a chunk walks all L levels before the next one starts.  Its good count, and so the
@@ -1760,25 +1809,20 @@ int refine_walk_impl(cotr_model* m, const uint8_t* const* images, const int32_t*
     *walked = 0;
     if (n == 0 || max_good <= 0) { m->launches = 0; return 0; }
 
-    // the Pillow coefficient tables of every crop side (uploaded once per side length), the per-level crop templates
-    if (!m->pre) m->pre = preprocessor_create();
+    // the per-level crop templates
     std::vector<RefineLevel> levels((size_t)n_groups * L);
     for (int g = 0; g < n_groups; ++g) {
         const cotr_refine_group& G = groups[g];
-        for (int l = 0; l < L; ++l) {
-            RefineLevel& lv = levels[(size_t)g * L + l];
-            lv = RefineLevel();
-            lv.level = l; lv.levels = L;
-            lv.h_from = hw[2 * G.image_from]; lv.w_from = hw[2 * G.image_from + 1];
-            lv.h_to = hw[2 * G.image_to]; lv.w_to = hw[2 * G.image_to + 1];
-            lv.thr = refine_threshold(rel, lv.h_to, lv.w_to);
-            lv.from.img = images[G.image_from]; lv.from.img_w = lv.w_from;
-            lv.to.img = images[G.image_to]; lv.to.img_w = lv.w_to;
-            if (preprocess_coeffs(m->pre, sizes[(g * L + l) * 2], &lv.from)) return 1;
-            if (preprocess_coeffs(m->pre, sizes[(g * L + l) * 2 + 1], &lv.to)) return 1;
-        }
+        const int a = G.image_from, b = G.image_to;
+        for (int l = 0; l < L; ++l)
+            if (refine_level_template(m, images[a], hw[2 * a], hw[2 * a + 1], images[b], hw[2 * b], hw[2 * b + 1], sizes[(g * L + l) * 2],
+                                      sizes[(g * L + l) * 2 + 1], l, L, rel, &levels[(size_t)g * L + l])) return 1;
     }
-    if (ensure_refine_ws(m, std::min<int64_t>(batch, n), tmp, n_chunks)) return 1;
+    // squads of one: chunk task i is entry i, squad i, rank 0
+    const int64_t rows = std::min<int64_t>(batch, n);
+    RefineCaps need;
+    need.squads = need.rows = need.ids = rows; need.tmp = tmp; need.chunks = n_chunks;
+    if (ensure_refine_ws(m, need)) return 1;
     Workspace& w = m->ws;
     int32_t* chunk_good = reinterpret_cast<int32_t*>(w.refine_counts + 1);
     COTR_CHECK_CUDA(cudaMemsetAsync(w.refine_counts, 0xFF, sizeof(unsigned long long), s));
@@ -1787,8 +1831,7 @@ int refine_walk_impl(cotr_model* m, const uint8_t* const* images, const int32_t*
     COTR_CHECK_CUDA(cudaMemcpy2DAsync(history, (size_t)(L + 1) * 2 * sizeof(double), loc_to, 2 * sizeof(double), 2 * sizeof(double),
                                       (size_t)n, cudaMemcpyDeviceToDevice, s));
 
-    Run r{m, s};
-    int launches = 0;
+    m->launches = 0;
     const bool look_each_wave = max_good < n;
     std::vector<int32_t> counts;
     int64_t good_so_far = 0;
@@ -1799,29 +1842,10 @@ int refine_walk_impl(cotr_model* m, const uint8_t* const* images, const int32_t*
             for (int l = 0; l < L; ++l) {
                 RefineLevel lv = levels[(size_t)ch.group * L + l];
                 lv.task0 = ch.first; lv.count = ch.count; lv.chunk = (int)c;
-                m->launches = 0;
-                {
-                    LaunchScope scope(r, K_REFINE_GEOMETRY, ch.count, l, 0);
-                    if (launch_refine_geometry(lv, loc_from, history, w.refine_sides, rects, w.refine_q, w.refine_counts, s)) return 1;
-                }
-                {
-                    LaunchScope scope(r, K_RESIZE_H, 2 * ch.count, 0, 0);
-                    if (launch_resize_h(w.refine_sides, 2 * ch.count, std::max(lv.from.size, lv.to.size), w.refine_tmp, s)) return 1;
-                }
-                {
-                    LaunchScope scope(r, K_RESIZE_V, 2 * ch.count, 0, 0);
-                    if (launch_resize_v(w.refine_sides, 2 * ch.count, w.refine_tmp, w.refine_canvas, s)) return 1;
-                }
-                launches += m->launches;
-                if (forward_eager(m, w.refine_canvas, w.refine_q, ch.count, 1, w.refine_pred, s)) return 1;
-                {
-                    LaunchScope scope(r, K_REFINE_STEP, ch.count, l, 0);
-                    if (launch_refine_step(lv, w.refine_pred, rects, history, good, chunk_good, w.refine_counts, s)) return 1;
-                }
-                launches += m->launches;
+                if (refine_level(m, lv, w.refine_iota, w.refine_iota, w.refine_zeros, ch.count, 1, true, loc_from, history, rects, good,
+                                 chunk_good + c, s)) return 1;
             }
         }
-        m->launches = launches;
         const bool last = w1 == n_chunks;
         if (!look_each_wave && !last) continue;
         // one small copy: the status word, then (when the stop may fall in this wave) the wave's good counts
@@ -1869,19 +1893,16 @@ int refine_grouped_impl(cotr_model* m, const uint8_t* img_from, int h_from, int 
     for (int k = 0; k < 5; ++k) result[k] = 0;
     m->launches = 0;
     if (n_ids == 0) return 0;
-    if (!m->pre) m->pre = preprocessor_create();
-    RefineLevel lv = RefineLevel();
-    lv.task0 = 0; lv.count = n_ids; lv.level = level; lv.levels = L; lv.chunk = 0;
-    lv.h_from = h_from; lv.w_from = w_from; lv.h_to = h_to; lv.w_to = w_to;
-    lv.thr = refine_threshold(rel, h_to, w_to);
-    lv.from.img = img_from; lv.from.img_w = w_from;
-    lv.to.img = img_to; lv.to.img_w = w_to;
-    if (preprocess_coeffs(m->pre, fs, &lv.from) || preprocess_coeffs(m->pre, ts, &lv.to)) return 1;
+    RefineLevel lv;
+    if (refine_level_template(m, img_from, h_from, w_from, img_to, h_to, w_to, fs, ts, level, L, rel, &lv)) return 1;
+    lv.count = n_ids;
     // every buffer at its largest for this batch before the first launch: growing one later would drop the squad table
-    const int64_t max_squads = std::min(batch_size, n_ids);
-    const int64_t max_rows = max_squads * std::min<int64_t>((int64_t)max_load + 1, n_ids);
-    if (ensure_refine_ws(m, (int)max_squads, (size_t)max_squads * (fs + ts) * 256 * 3, 0)) return 1;
-    if (ensure_grouped_ws(m, n_ids, max_rows)) return 1;
+    RefineCaps need;
+    need.squads = std::min(batch_size, n_ids);
+    need.rows = need.squads * std::min<int64_t>((int64_t)max_load + 1, n_ids);
+    need.ids = n_ids;
+    need.tmp = (size_t)need.squads * (fs + ts) * 256 * 3;
+    if (ensure_refine_ws(m, need)) return 1;
     if (m->grouped_ids.upload(ids_host, (size_t)n_ids, s)) return 1;
     Workspace& w = m->ws;
     const int32_t* ids = m->grouped_ids.dev;
@@ -1922,28 +1943,9 @@ int refine_grouped_impl(cotr_model* m, const uint8_t* img_from, int h_from, int 
     result[0] = n_squads; result[1] = longest; result[2] = num_steps; result[4] = status;
     if (status != 0 || n_squads == 0) return 0;
     const bool step = !(max_good <= 0 || (read_good && good_count >= max_good));
-    COTR_CHECK_CUDA(cudaMemsetAsync(w.grouped_q, 0, (size_t)n_squads * longest * 2 * sizeof(float), s));    // padding rows
-    {
-        LaunchScope scope(r, K_GROUPED_GEOMETRY, n_ids, level, 0);
-        if (launch_grouped_geometry(lv, ids, squad, rank, n_squads, longest, loc_from, history, w.refine_sides, rects, w.grouped_q, s)) return 1;
-    }
-    if (!step) return 0;
-    {
-        LaunchScope scope(r, K_RESIZE_H, 2 * n_squads, 0, 0);
-        if (launch_resize_h(w.refine_sides, 2 * n_squads, std::max(fs, ts), w.refine_tmp, s)) return 1;
-    }
-    {
-        LaunchScope scope(r, K_RESIZE_V, 2 * n_squads, 0, 0);
-        if (launch_resize_v(w.refine_sides, 2 * n_squads, w.refine_tmp, w.refine_canvas, s)) return 1;
-    }
-    const int launches = m->launches;     // forward_eager counts its own launches from 0
-    if (forward_eager(m, w.refine_canvas, w.grouped_q, n_squads, longest, w.grouped_pred, s)) return 1;
-    {
-        LaunchScope scope(r, K_GROUPED_STEP, n_ids, level, 0);
-        if (launch_grouped_step(lv, ids, squad, rank, longest, w.grouped_pred, rects, history, good, good + n_tasks, s)) return 1;
-    }
-    m->launches += launches;
-    result[3] = 1;
+    COTR_CHECK_CUDA(cudaMemsetAsync(w.refine_q, 0, (size_t)n_squads * longest * 2 * sizeof(float), s));    // padding rows
+    if (refine_level(m, lv, ids, squad, rank, n_squads, longest, step, loc_from, history, rects, good, good + n_tasks, s)) return 1;
+    result[3] = step;
     return 0;
 }
 
@@ -2023,15 +2025,12 @@ int cotr_refine(cotr_model* m, const uint8_t* const* images_host, const int32_t*
                    fn, g, G.first, G.count);
         n += G.count;
         COTR_CHECK(n <= INT32_MAX, "%s: more than %d tasks", fn, INT32_MAX);
+        char where[48];
+        snprintf(where, sizeof(where), "%s: group %d", fn, g);
+        const int a = G.image_from, b = G.image_to;
         for (int l = 0; l < n_zoom; ++l)
-            for (int side = 0; side < 2; ++side) {
-                const int img = side ? G.image_to : G.image_from;
-                const int h = hw_host[2 * img], w = hw_host[2 * img + 1];
-                const int size = refine_crop_size(h, w, (side ? G.s_to : G.s_from) * zoom_host[l]);
-                COTR_CHECK(size >= 2 && size <= h && size <= w, "%s: group %d level %d: %s crop side %d in a %d x %d image", fn, g, l,
-                           side ? "to" : "from", size, h, w);
-                sizes[((size_t)g * n_zoom + l) * 2 + side] = size;
-            }
+            if (refine_crop_sides(where, l, zoom_host[l], hw_host[2 * a], hw_host[2 * a + 1], G.s_from, hw_host[2 * b], hw_host[2 * b + 1],
+                                  G.s_to, &sizes[((size_t)g * n_zoom + l) * 2])) return 1;
     }
     COTR_CHECK(loc_from_dev && loc_to_dev && history_dev && rects_dev && good_dev, "%s: null device buffer", fn);
     COTR_CHECK(((uintptr_t)loc_from_dev & 7) == 0 && ((uintptr_t)loc_to_dev & 7) == 0 && ((uintptr_t)history_dev & 7) == 0,
@@ -2066,12 +2065,7 @@ int cotr_refine_grouped(cotr_model* m, const uint8_t* img_from_dev, int h_from, 
         seen[t] = 1;
     }
     int sizes[2];
-    for (int side = 0; side < 2; ++side) {
-        const int h = side ? h_to : h_from, w = side ? w_to : w_from;
-        sizes[side] = refine_crop_size(h, w, (side ? s_to : s_from) * zoom_host[level]);
-        COTR_CHECK(sizes[side] >= 2 && sizes[side] <= h && sizes[side] <= w, "%s: level %d: %s crop side %d in a %d x %d image", fn, level,
-                   side ? "to" : "from", sizes[side], h, w);
-    }
+    if (refine_crop_sides(fn, level, zoom_host[level], h_from, w_from, s_from, h_to, w_to, s_to, sizes)) return 1;
     COTR_CHECK(loc_from_dev && history_dev && rects_dev && good_dev, "%s: null device buffer", fn);
     COTR_CHECK(((uintptr_t)loc_from_dev & 7) == 0 && ((uintptr_t)history_dev & 7) == 0, "%s: loc_from_dev or history_dev is not 8-byte aligned", fn);
     COTR_CHECK(((uintptr_t)rects_dev & 3) == 0 && ((uintptr_t)good_dev & 3) == 0, "%s: rects_dev or good_dev is not 4-byte aligned", fn);

@@ -1,8 +1,9 @@
-// The zoom-in walk of cotr_refine (include/cotr_b200.h): the per-task arithmetic of RefinementTask with
-// converge_iters = 1 (refinement_task.py, inference_helper.py:79-96) - crop geometry, canvas query, scale_to_loc and
-// conclude() - as numpy / Python evaluate it, bit for bit.  The functions below are __host__ __device__: the kernels use
-// them with explicit round-to-nearest intrinsics (no contraction), and cotr_test_refine_math runs the same code on the
-// host (plain IEEE double / float arithmetic, no FMA on the x86-64 baseline) so that it can be checked against Python.
+// The zoom-in walks of cotr_refine and cotr_refine_grouped (include/cotr_b200.h): the per-task arithmetic of
+// RefinementTask with converge_iters = 1 (refinement_task.py, inference_helper.py:79-96) - crop geometry, canvas query,
+// scale_to_loc and conclude() - as numpy / Python evaluate it, bit for bit.  The functions below are __host__ __device__:
+// the kernels use them with explicit round-to-nearest intrinsics (no contraction), and cotr_test_refine_math runs the
+// same code on the host (plain IEEE double / float arithmetic, no FMA on the x86-64 baseline) so that it can be checked
+// against Python.
 #include <cmath>
 
 #include "../../include/cotr_b200.h"
@@ -117,56 +118,6 @@ __device__ inline unsigned long long status_key(const RefineLevel& lv, int code)
     return ((unsigned long long)lv.chunk * 8 + (unsigned long long)lv.level) * 4 + (unsigned long long)code;
 }
 
-__global__ void __launch_bounds__(128) refine_geometry_kernel(RefineLevel lv, const double* __restrict__ loc_from,
-                                                              const double* __restrict__ history, CropSide* __restrict__ sides,
-                                                              int32_t* __restrict__ rects, float* __restrict__ queries,
-                                                              unsigned long long* __restrict__ status) {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= lv.count) return;
-    const size_t t = (size_t)lv.task0 + i;
-    const double* lf = loc_from + 2 * t;
-    const double* lt = history + (t * (lv.levels + 1) + lv.level) * 2;
-    const int fs = lv.from.size, ts = lv.to.size;
-    int flag = 0;
-    CropSide a = lv.from, b = lv.to;
-    a.x = patch_corner(lf[0], fs, lv.w_from, &flag);
-    a.y = patch_corner(lf[1], fs, lv.h_from, &flag);
-    b.x = patch_corner(lt[0], ts, lv.w_to, &flag);
-    b.y = patch_corner(lt[1], ts, lv.h_to, &flag);
-    // horizontal-pass bytes: the chunk's "from" crops first, then its "to" crops
-    a.tmp_offset = (size_t)i * fs * 256 * 3;
-    b.tmp_offset = (size_t)lv.count * fs * 256 * 3 + (size_t)i * ts * 256 * 3;
-    sides[2 * i] = a;
-    sides[2 * i + 1] = b;
-    int32_t* r = rects + (t * lv.levels + lv.level) * 6;
-    r[0] = a.x; r[1] = a.y; r[2] = fs; r[3] = b.x; r[4] = b.y; r[5] = ts;
-    const float2 q = query_in(lf[0], lf[1], a.x, a.y, fs);
-    queries[2 * i] = q.x;
-    queries[2 * i + 1] = q.y;
-    if (flag) atomicMin(status, status_key(lv, 2));
-}
-
-__global__ void __launch_bounds__(128) refine_step_kernel(RefineLevel lv, const float* __restrict__ pred,
-                                                          const int32_t* __restrict__ rects, double* __restrict__ history,
-                                                          int32_t* __restrict__ good, int32_t* __restrict__ chunk_good,
-                                                          unsigned long long* __restrict__ status) {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= lv.count) return;
-    const size_t t = (size_t)lv.task0 + i;
-    const float p = pred[2 * i], q = pred[2 * i + 1];
-    if (p != p || q != q) atomicMin(status, status_key(lv, 1));
-    const int32_t* r = rects + (t * lv.levels + lv.level) * 6;
-    const double2 loc = scale_to_loc(p, q, r[3], r[4], r[5]);
-    double* h = history + t * (lv.levels + 1) * 2;
-    h[2 * (lv.level + 1)] = loc.x;
-    h[2 * (lv.level + 1) + 1] = loc.y;
-    if (lv.level == lv.levels - 1) {
-        const bool g = conclude_good(h, lv.levels + 1, lv.thr);
-        good[t] = g ? 1 : 0;
-        if (g) atomicAdd(chunk_good + lv.chunk, 1);
-    }
-}
-
 // ---- grouped walk (cotr_refine_grouped): FasterSparseEngine's squads at one level ----------------------------------
 
 // Corner of a candidate's pilot box as FasterSparseEngine._pilot_boxes computes it: np.trunc(pos - size // 2) cast to
@@ -223,39 +174,47 @@ __global__ void __launch_bounds__(128) grouped_candidates_kernel(RefineLevel lv,
     fail[i] = crop_failure(lt[0], lt[1], crop_failure(lf[0], lf[1], 0));
 }
 
+// ---- one level of either walk: entry i is task lv.task0 + ids[i] in squad squad[i] at rank rank[i] -----------------
+// cotr_refine's tasks are squads of one (ids = squad = 0 .. count-1, rank = 0, longest = 1, task0 = the chunk's first
+// task); cotr_refine_grouped's are the candidates of one batch (task0 = 0, squad -1 for the ones left out).
+
 // One CTA per squad: the pilot's crops (get_patch_centered_at) become CropSide 2s / 2s+1 and the rect of this level of
 // every member (the pilot's two patches, as get_task_pilot submits them), and each member's canvas query is its own
 // loc_from in the pilot's "from" patch, at row s * longest + rank (pilot first, then the members in list order).
-__global__ void __launch_bounds__(256) grouped_geometry_kernel(RefineLevel lv, const int32_t* __restrict__ ids,
-                                                               const int32_t* __restrict__ squad, const int32_t* __restrict__ rank,
-                                                               int n_squads, int longest, const double* __restrict__ loc_from,
-                                                               const double* __restrict__ history, CropSide* __restrict__ sides,
-                                                               int32_t* __restrict__ rects, float* __restrict__ queries) {
+// Non-finite pilot positions flag `status`; cotr_refine_grouped never gets there, since it stops at such a pilot.
+__global__ void __launch_bounds__(256) refine_geometry_kernel(RefineLevel lv, const int32_t* __restrict__ ids,
+                                                              const int32_t* __restrict__ squad, const int32_t* __restrict__ rank,
+                                                              int n_squads, int longest, const double* __restrict__ loc_from,
+                                                              const double* __restrict__ history, CropSide* __restrict__ sides,
+                                                              int32_t* __restrict__ rects, float* __restrict__ queries,
+                                                              unsigned long long* __restrict__ status) {
     __shared__ int s_rect[4];
     const int s = blockIdx.x;
     const int fs = lv.from.size, ts = lv.to.size;
     for (int i = threadIdx.x; i < lv.count; i += blockDim.x) {
         if (squad[i] != s || rank[i] != 0) continue;
-        const size_t t = (size_t)ids[i];
+        const size_t t = (size_t)lv.task0 + ids[i];
         const double* lf = loc_from + 2 * t;
         const double* lt = history + (t * (lv.levels + 1) + lv.level) * 2;
-        int flag = 0;       // a non-finite pilot position was reported by grouped_candidates_kernel; the call stops first
+        int flag = 0;
         CropSide a = lv.from, b = lv.to;
         a.x = patch_corner(lf[0], fs, lv.w_from, &flag);
         a.y = patch_corner(lf[1], fs, lv.h_from, &flag);
         b.x = patch_corner(lt[0], ts, lv.w_to, &flag);
         b.y = patch_corner(lt[1], ts, lv.h_to, &flag);
+        // horizontal-pass bytes: the level's "from" crops first, then its "to" crops
         a.tmp_offset = (size_t)s * fs * 256 * 3;
         b.tmp_offset = (size_t)n_squads * fs * 256 * 3 + (size_t)s * ts * 256 * 3;
         sides[2 * s] = a;
         sides[2 * s + 1] = b;
         s_rect[0] = a.x; s_rect[1] = a.y; s_rect[2] = b.x; s_rect[3] = b.y;
+        if (flag) atomicMin(status, status_key(lv, 2));
     }
     __syncthreads();
     const int ax = s_rect[0], ay = s_rect[1], bx = s_rect[2], by = s_rect[3];
     for (int i = threadIdx.x; i < lv.count; i += blockDim.x) {
         if (squad[i] != s) continue;
-        const size_t t = (size_t)ids[i];
+        const size_t t = (size_t)lv.task0 + ids[i];
         int32_t* r = rects + (t * lv.levels + lv.level) * 6;
         r[0] = ax; r[1] = ay; r[2] = fs; r[3] = bx; r[4] = by; r[5] = ts;
         const float2 q = query_in(loc_from[2 * t], loc_from[2 * t + 1], ax, ay, fs);
@@ -266,15 +225,17 @@ __global__ void __launch_bounds__(256) grouped_geometry_kernel(RefineLevel lv, c
 }
 
 // RefinementTask.step for every member: scale_to_loc with its pilot's "to" patch into history row level + 1; at the
-// last level conclude(), the good flag and good[n] += 1.
-__global__ void __launch_bounds__(128) grouped_step_kernel(RefineLevel lv, const int32_t* __restrict__ ids, const int32_t* __restrict__ squad,
-                                                           const int32_t* __restrict__ rank, int longest, const float* __restrict__ pred,
-                                                           const int32_t* __restrict__ rects, double* __restrict__ history,
-                                                           int32_t* __restrict__ good, int32_t* __restrict__ good_count) {
+// last level conclude(), the good flag and *good_count += 1.  A NaN prediction flags `status`.
+__global__ void __launch_bounds__(128) refine_step_kernel(RefineLevel lv, const int32_t* __restrict__ ids, const int32_t* __restrict__ squad,
+                                                          const int32_t* __restrict__ rank, int longest, const float* __restrict__ pred,
+                                                          const int32_t* __restrict__ rects, double* __restrict__ history,
+                                                          int32_t* __restrict__ good, int32_t* __restrict__ good_count,
+                                                          unsigned long long* __restrict__ status) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= lv.count || squad[i] < 0) return;
-    const size_t t = (size_t)ids[i];
+    const size_t t = (size_t)lv.task0 + ids[i];
     const float* p = pred + ((size_t)squad[i] * longest + rank[i]) * 2;
+    if (p[0] != p[0] || p[1] != p[1]) atomicMin(status, status_key(lv, 1));
     const int32_t* r = rects + (t * lv.levels + lv.level) * 6;
     const double2 loc = scale_to_loc(p[0], p[1], r[3], r[4], r[5]);
     double* h = history + t * (lv.levels + 1) * 2;
@@ -306,22 +267,6 @@ double refine_threshold(double rel, int h_to, int w_to) {
     return rel * (double)mx;
 }
 
-int launch_refine_geometry(const RefineLevel& lv, const double* loc_from, const double* history, CropSide* sides,
-                           int32_t* rects, float* queries, unsigned long long* status, cudaStream_t s) {
-    refine_geometry_kernel<<<(lv.count + kRefineThreads - 1) / kRefineThreads, kRefineThreads, 0, s>>>(lv, loc_from, history, sides,
-                                                                                                      rects, queries, status);
-    COTR_CHECK_CUDA(cudaGetLastError());
-    return 0;
-}
-
-int launch_refine_step(const RefineLevel& lv, const float* pred, const int32_t* rects, double* history, int32_t* good,
-                       int32_t* chunk_good, unsigned long long* status, cudaStream_t s) {
-    refine_step_kernel<<<(lv.count + kRefineThreads - 1) / kRefineThreads, kRefineThreads, 0, s>>>(lv, pred, rects, history, good,
-                                                                                                  chunk_good, status);
-    COTR_CHECK_CUDA(cudaGetLastError());
-    return 0;
-}
-
 int launch_grouped_candidates(const RefineLevel& lv, const int32_t* ids, const double* loc_from, const double* history, double* pts,
                               double* box, int32_t* fail, cudaStream_t s) {
     grouped_candidates_kernel<<<(lv.count + kRefineThreads - 1) / kRefineThreads, kRefineThreads, 0, s>>>(lv, ids, loc_from, history,
@@ -330,18 +275,20 @@ int launch_grouped_candidates(const RefineLevel& lv, const int32_t* ids, const d
     return 0;
 }
 
-int launch_grouped_geometry(const RefineLevel& lv, const int32_t* ids, const int32_t* squad, const int32_t* rank, int n_squads,
-                            int longest, const double* loc_from, const double* history, CropSide* sides, int32_t* rects,
-                            float* queries, cudaStream_t s) {
-    grouped_geometry_kernel<<<n_squads, 256, 0, s>>>(lv, ids, squad, rank, n_squads, longest, loc_from, history, sides, rects, queries);
+int launch_refine_geometry(const RefineLevel& lv, const int32_t* ids, const int32_t* squad, const int32_t* rank, int n_squads,
+                           int longest, const double* loc_from, const double* history, CropSide* sides, int32_t* rects,
+                           float* queries, unsigned long long* status, cudaStream_t s) {
+    refine_geometry_kernel<<<n_squads, 256, 0, s>>>(lv, ids, squad, rank, n_squads, longest, loc_from, history, sides, rects, queries,
+                                                    status);
     COTR_CHECK_CUDA(cudaGetLastError());
     return 0;
 }
 
-int launch_grouped_step(const RefineLevel& lv, const int32_t* ids, const int32_t* squad, const int32_t* rank, int longest,
-                        const float* pred, const int32_t* rects, double* history, int32_t* good, int32_t* good_count, cudaStream_t s) {
-    grouped_step_kernel<<<(lv.count + kRefineThreads - 1) / kRefineThreads, kRefineThreads, 0, s>>>(lv, ids, squad, rank, longest, pred,
-                                                                                                   rects, history, good, good_count);
+int launch_refine_step(const RefineLevel& lv, const int32_t* ids, const int32_t* squad, const int32_t* rank, int longest,
+                       const float* pred, const int32_t* rects, double* history, int32_t* good, int32_t* good_count,
+                       unsigned long long* status, cudaStream_t s) {
+    refine_step_kernel<<<(lv.count + kRefineThreads - 1) / kRefineThreads, kRefineThreads, 0, s>>>(lv, ids, squad, rank, longest, pred,
+                                                                                                  rects, history, good, good_count, status);
     COTR_CHECK_CUDA(cudaGetLastError());
     return 0;
 }

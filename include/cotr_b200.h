@@ -232,9 +232,9 @@ int cotr_refine(cotr_model* m, const uint8_t* const* images_host, const int32_t*
  *   to even must be >= 2.  loc_from_dev: n_tasks x 2 fp64; history_dev: n_tasks x (L+1) x 2 fp64 (row 0 = first guesses,
  *   filled by the caller); rects_dev: n_tasks x L x 6 int32 as in cotr_refine; good_dev: n_tasks + 1 int32 (the caller
  *   zeroes the count before the first batch).  L = n_zoom, 1 .. 7.  Every argument is checked before anything is
- *   enqueued; the candidate tables, queries and predictions are model-owned and grow on demand, and the canvases are
- *   cotr_refine's.  Launches: grouped_candidates, group_tasks, then grouped_geometry, and when stepped resize_h,
- *   resize_v, the forward, grouped_step. */
+ *   enqueued; the candidate tables, canvases, queries and predictions are model-owned, shared with cotr_refine, and grow
+ *   on demand.  Launches: grouped_candidates, group_tasks, then refine_geometry, and when stepped resize_h, resize_v,
+ *   the forward, refine_step: the level launches of cotr_refine, with squads in place of single tasks. */
 int cotr_refine_grouped(cotr_model* m, const uint8_t* img_from_dev, int h_from, int w_from, const uint8_t* img_to_dev, int h_to,
                         int w_to, double s_from, double s_to, const double* zoom_host, int n_zoom, int level, const int32_t* ids_host,
                         int n_ids, int n_tasks, int batch_size, int max_load, int64_t max_good, double rel_threshold,
@@ -324,10 +324,11 @@ int cotr_last_launch_count(const cotr_model* m);
  * kernel ids: 0 gemm_tc (wgmma), 1 gemm_simt, 2 attention_tc, 3 attention_simt, 4 layernorm, 5 maxpool,
  * 6 query_encode, 7 stem_canvas, 8 gemm_mlp (fused feed-forward block), 9 attention_weights_tc, 10 attention_weights_simt
  * (the maps of cotr_*_attention), 11 match_queries, 12 match_pixels, 13 nearest, 14 mutual (cotr_match_keypoints),
- * 15 refine_geometry, 16 resize_h, 17 resize_v, 18 refine_step (cotr_refine), 19 grouped_candidates, 20 group_tasks,
- * 21 grouped_geometry, 22 grouped_step (cotr_refine_grouped, with 16-17).  For GEMMs M,N,K are the problem size; for
- * attention and attention weights M = query rows, N = 512, K = 256; for 11-13 M = rows, N = 2; for 14 M = pairs; for 15
- * and 18 M = tasks, N = level; for 16-17 M = crops; for 19-22 M = candidates, N = level. */
+ * 15 refine_geometry, 16 resize_h, 17 resize_v, 18 refine_step (cotr_refine and cotr_refine_grouped),
+ * 19 grouped_candidates, 20 group_tasks (cotr_refine_grouped).  For GEMMs M,N,K are the problem size; for attention and
+ * attention weights M = query rows, N = 512, K = 256; for 11-13 M = rows, N = 2; for 14 M = pairs; for 15 and 18
+ * M = tasks of the launch (cotr_refine_grouped: its candidates), N = level; for 16-17 M = crops; for 19-20
+ * M = candidates, N = level. */
 typedef struct cotr_launch_record {
     int32_t kernel;
     int32_t M, N, K;

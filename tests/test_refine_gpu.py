@@ -282,3 +282,43 @@ def test_nan_prediction_raises_on_both_paths(built_lib, images, capsys):
             _engine(model, 16, walk)._single_query_loop(_tasks(img_a, img_b, lf, lt, AREAS, ZOOMS), 40)
         out.append(capsys.readouterr().out)
     assert out[0] == out[1]
+
+
+def test_level_launch_sequence(native, images):
+    """Both walks run each level as refine_geometry, resize_h, resize_v, the forward's launches at (squads, longest) and
+    refine_step: cotr_refine with squads of one task, cotr_refine_grouped with the squads of its batch."""
+    nat = native.native()
+    dev_a, dev_b = (torch.from_numpy(np.ascontiguousarray(i)).cuda() for i in images)
+    rs = np.random.RandomState(29)
+    n, zooms = 12, [0.5, 0.25]
+    # clustered points: every task lies inside its pilot's boxes, so the grouped batch forms squads of several members
+    lf = torch.from_numpy(150 + rs.uniform(-5, 5, (n, 2))).cuda()
+    lt = torch.from_numpy(200 + rs.uniform(-5, 5, (n, 2))).cuda()
+
+    def forward(B, Q):
+        nat.profile_begin()
+        nat.forward(torch.zeros((B, 3, 256, 512), device="cuda"), torch.full((B, Q, 2), 0.5, device="cuda"))
+        return [r[:4] for r in nat.profile_end()]
+
+    def level(entries, l, n_squads, longest):
+        return ([("refine_geometry", entries, l, 0), ("resize_h", 2 * n_squads, 0, 0), ("resize_v", 2 * n_squads, 0, 0)] +
+                forward(n_squads, longest) + [("refine_step", entries, l, 0)])
+
+    expect = [rec for count in (8, 4) for l in range(len(zooms)) for rec in level(count, l, count, 1)]
+    nat.profile_begin()
+    _, _, _, walked, status = nat.refine([dev_a, dev_b], [(0, 1, 0, n, 1.0, 1.0)], zooms, 8, 4, n, 0.02, lf, lt)
+    rec = [r[:4] for r in nat.profile_end()]
+    assert walked == n and status == (0, 0, 0)
+    assert rec == expect and nat.last_launch_count() == len(rec)
+
+    history = torch.zeros((n, len(zooms) + 1, 2), dtype=torch.float64, device="cuda")
+    history[:, 0] = lt
+    rects = torch.zeros((n, len(zooms), 6), dtype=torch.int32, device="cuda")
+    good = torch.zeros((n + 1,), dtype=torch.int32, device="cuda")
+    nat.profile_begin()
+    squad, (n_squads, longest, steps, stepped, fail) = nat.refine_grouped(dev_a, dev_b, 1.0, 1.0, zooms, 0, rs.permutation(n), 4, 3,
+                                                                          10 ** 6, 0.02, lf, history, rects, good)
+    rec = [r[:4] for r in nat.profile_end()]
+    assert stepped == 1 and fail == 0 and steps == n and longest > 1
+    assert nat.last_launch_count() == len(rec)
+    assert rec == [("grouped_candidates", n, 0, 0), ("group_tasks", n, 0, 0)] + level(n, 0, n_squads, longest)
