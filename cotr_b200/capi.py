@@ -51,7 +51,7 @@ class LaunchRecord(ctypes.Structure):
 
 KERNEL_NAMES = ("gemm_tc", "gemm_simt", "attention_tc", "attention_simt", "layernorm", "maxpool", "query_encode", "stem_canvas", "gemm_mlp",
                 "attention_weights_tc", "attention_weights_simt", "match_queries", "match_pixels", "nearest", "mutual",
-                "refine_geometry", "resize_h", "resize_v", "refine_step", "grouped_candidates", "group_tasks")
+                "refine_geometry", "resize_h", "resize_v", "refine_step", "grouped_candidates", "group_tasks", "dense_first_guess")
 
 # name -> (restype, argtypes); every symbol include/cotr_b200.h declares
 _PROTOTYPES = {
@@ -91,6 +91,9 @@ _PROTOTYPES = {
                              [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p]),
     "cotr_group_tasks": (ctypes.c_int, [ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int,
                                         ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]),
+    "cotr_dense_first_guess": (ctypes.c_int, [ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_void_p,
+                                              ctypes.c_int, ctypes.c_int, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_void_p,
+                                              ctypes.c_void_p, ctypes.c_void_p]),
     "cotr_rasterize_triangles": (ctypes.c_int, [ctypes.c_int, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p]),
     "cotr_exchange_create": (ctypes.c_int, [ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_size_t, ctypes.c_int, ctypes.POINTER(ctypes.c_void_p)]),
     "cotr_exchange_handle": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p]),
@@ -516,6 +519,24 @@ def mutual_nearest(kpts, kpt_offsets, pairs, corr):
     check(lib().cotr_mutual_nearest(dev, _ptr(kpts), ctypes.c_void_p(off.ctypes.data), off.size - 1, ctypes.c_void_p(pairs.ctypes.data),
                                     pairs.shape[0], _ptr(corr), _ptr(nearest), _ptr(match), _ptr(count), stream), "cotr_mutual_nearest")
     return nearest, match, count
+
+
+def dense_first_guess(flow, conf_from, conf_to, kpts, loc_to, counts):
+    """The forced first guesses of one direction (cotr_dense_first_guess).  flow (H_f,W_f,2) / conf_from (H_f,W_f) /
+    conf_to (H_t,W_t): contiguous fp32 CUDA maps; kpts (n,2) float32 or float64 CUDA (x, y); outputs written in place:
+    loc_to (n,2) fp64, counts (2,) int64 (pixels below THRESHOLD_AREA in conf_from, conf_to)."""
+    for t in (flow, conf_from, conf_to, kpts, loc_to, counts):
+        assert t.is_cuda and t.is_contiguous() and t.device == flow.device
+    assert flow.dtype == conf_from.dtype == conf_to.dtype == torch.float32 and kpts.dtype in (torch.float32, torch.float64)
+    assert flow.ndim == 3 and flow.shape[2] == 2 and tuple(conf_from.shape) == tuple(flow.shape[:2]) and conf_to.ndim == 2
+    n = kpts.shape[0]
+    assert kpts.shape == (n, 2) and loc_to.dtype == torch.float64 and loc_to.shape == (n, 2)
+    assert counts.dtype == torch.int64 and counts.shape == (2,)
+    dev = flow.device.index if flow.device.index is not None else torch.cuda.current_device()
+    stream = ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+    check(lib().cotr_dense_first_guess(dev, _ptr(flow), _ptr(conf_from), flow.shape[0], flow.shape[1], _ptr(conf_to), conf_to.shape[0],
+                                       conf_to.shape[1], _ptr(kpts), int(kpts.dtype == torch.float32), n, _ptr(loc_to), _ptr(counts),
+                                       stream), "cotr_dense_first_guess")
 
 
 def rasterize_triangles(tris, H, W):

@@ -385,7 +385,7 @@ struct Run {
 enum KernelId { K_GEMM_TC = 0, K_GEMM_SIMT = 1, K_ATTN_TC = 2, K_ATTN_SIMT = 3, K_LAYERNORM = 4, K_MAXPOOL = 5, K_QENC = 6, K_STEM_CANVAS = 7,
                 K_GEMM_MLP = 8, K_ATTN_WEIGHTS_TC = 9, K_ATTN_WEIGHTS_SIMT = 10, K_MATCH_QUERIES = 11, K_MATCH_PIXELS = 12,
                 K_NEAREST = 13, K_MUTUAL = 14, K_REFINE_GEOMETRY = 15, K_RESIZE_H = 16, K_RESIZE_V = 17, K_REFINE_STEP = 18,
-                K_GROUPED_CANDIDATES = 19, K_GROUP_TASKS = 20 };
+                K_GROUPED_CANDIDATES = 19, K_GROUP_TASKS = 20, K_DENSE_FIRST_GUESS = 21 };
 
 // Counts the launch and, when the profiler is on, brackets it with two events on the launching stream.
 struct LaunchScope {

@@ -189,9 +189,12 @@ def _affine_terms(to):
     return [to[0, 0], to[1, 0], to[0, 2], to[0, 1], to[1, 1], to[1, 2]]
 
 
-def _cotr_flow_device(model, patches_a, patches_b):
-    """cotr_patch_flow_exhaustive + merge_flow_patches with every per-tile array left on the device: the dense pass'
-    (256,512,3) answer is split into its halves by pointer, mapped / resized / merged by cotr_flow_tile_merge."""
+def dense_flow_maps(model, img_a_dev, img_b_dev, patches_a, patches_b):
+    """cotr_patch_flow_exhaustive + merge_flow_patches with every per-tile array left on the device: the tile canvases
+    are cut and resized by cotr_preprocess (bit for bit the PIL canvases of _to_network_canvas), the dense pass'
+    (256,512,3) answer is split into its halves by pointer, mapped / resized / merged by cotr_flow_tile_merge.
+    img_*_dev: uint8 HWC CUDA images; patches_*: their to_square_patches.  -> ((flow_a (H_a,W_a,2), conf_a (H_a,W_a)),
+    (flow_b, conf_b)) fp32 device tensors."""
     device = _model_device(model)
     unit = np.array([[-1, -1], [1, -1], [1, 1]], dtype=np.float32)
     canv = {}
@@ -201,7 +204,8 @@ def _cotr_flow_device(model, patches_a, patches_b):
     queries = torch.from_numpy(_dense_grid().reshape(-1, 2))[None].float().to(device)
     for p_i in patches_a:
         for p_j in patches_b:
-            img = _to_network_canvas(p_i.patch, p_j.patch)[None].to(device)
+            rect = np.array([[p_i.x, p_i.y, p_i.w, p_j.x, p_j.y, p_j.w]], dtype=np.int32)
+            img = model.preprocess_canvases(img_a_dev, img_b_dev, rect)
             pred = model.forward(img, queries)['pred_corrs'].detach()
             corr = model.dense_postprocess(pred)[0]                           # (256,512,3) on the device
             to_j = cv2.getAffineTransform(unit, _patch_corners_ndc(p_j))
@@ -209,19 +213,28 @@ def _cotr_flow_device(model, patches_a, patches_b):
             model.flow_tile_merge(corr[:, :MAX_SIZE, :], _affine_terms(to_j), p_i, canv["a"][0], canv["a"][1], first)
             model.flow_tile_merge(corr[:, MAX_SIZE:, :], _affine_terms(to_i), p_j, canv["b"][0], canv["b"][1], first)
             first = False
-    out = []
-    for key in ("a", "b"):
-        flow, conf = canv[key]
-        out.append((flow.cpu().numpy().astype(np.float64), conf.cpu().numpy().astype(np.float64)))   # the reference's arrays are float64
-    return out
+    return canv["a"], canv["b"]
+
+
+def _cotr_flow_device(model, img_a, img_b, patches_a, patches_b):
+    device = _model_device(model)
+    maps = dense_flow_maps(model, torch.from_numpy(np.ascontiguousarray(img_a)).to(device),
+                           torch.from_numpy(np.ascontiguousarray(img_b)).to(device), patches_a, patches_b)
+    # the reference's arrays are float64
+    return [(flow.cpu().numpy().astype(np.float64), conf.cpu().numpy().astype(np.float64)) for flow, conf in maps]
+
+
+def _device_pixels(img):
+    return isinstance(img, np.ndarray) and img.dtype == np.uint8 and img.ndim == 3 and img.shape[2] == 3
 
 
 def cotr_flow(model, img_a, img_b):
     """Dense correspondence maps in [-1,1] + cycle confidence + warped images, both directions (:168-182)."""
     patches_a, patches_b = to_square_patches(img_a), to_square_patches(img_b)
     if (LARGE_GPU and DEVICE_DENSE_POST and DEVICE_FLOW_MERGE and hasattr(model, 'flow_tile_merge') and hasattr(model, 'dense_postprocess')
+            and hasattr(model, 'preprocess_canvases') and _device_pixels(img_a) and _device_pixels(img_b)
             and _model_device(model).type == 'cuda'):
-        (corr_a, con_a), (corr_b, con_b) = _cotr_flow_device(model, patches_a, patches_b)
+        (corr_a, con_a), (corr_b, con_b) = _cotr_flow_device(model, img_a, img_b, patches_a, patches_b)
     else:
         corrs_a, corrs_b = cotr_patch_flow_exhaustive(model, patches_a, patches_b)
         corr_a, con_a, _ = merge_flow_patches(corrs_a)

@@ -18,6 +18,14 @@ def _geometry_only(p):
     return ImagePatch(None, p.x, p.y, p.w, p.h, p.ow, p.oh)
 
 
+def crop_scales(area_from, area_to):
+    """(s_from, s_to): the image with the larger co-visible area gets the larger crop (refinement_task.py:25-30).  With
+    numpy float64 areas an area of 0 gives an infinite scale, and two give NaN, as in the reference."""
+    if area_from < area_to:
+        return BASE_ZOOM, BASE_ZOOM * np.sqrt(area_to / area_from)
+    return BASE_ZOOM * np.sqrt(area_from / area_to), BASE_ZOOM
+
+
 class RefinementTask():
     def __init__(self, image_from, image_to, loc_from, loc_to, area_from, area_to, converge_iters, zoom_ins, identifier=None):
         self.identifier = identifier
@@ -28,13 +36,7 @@ class RefinementTask():
         self.cur_loc_to = loc_to
         self.area_from = area_from
         self.area_to = area_to
-        # the image with the larger co-visible area gets the larger crop (refinement_task.py:25-30)
-        if area_from < area_to:
-            self.s_from = BASE_ZOOM
-            self.s_to = BASE_ZOOM * np.sqrt(area_to / area_from)
-        else:
-            self.s_to = BASE_ZOOM
-            self.s_from = BASE_ZOOM * np.sqrt(area_from / area_to)
+        self.s_from, self.s_to = crop_scales(area_from, area_to)
         self.cur_job = {}
         self.status = 'unfinished'
         self.result = 'unknown'

@@ -258,6 +258,22 @@ int cotr_dense_postprocess(cotr_model* m, const float* pred_dev, int n, float* o
 int cotr_flow_tile_merge(cotr_model* m, const float* tile_dev, int pitch_floats, const double* affine_host, int px, int py, int pw, int ph,
                          int ow, int oh, float* flow_dev, float* conf_dev, int first, void* cuda_stream);
 
+/* The first guesses of the forced zoom-in for ONE direction, from its merged dense maps (the `force` branch of
+ * SparseEngine.gen_tasks, COTR/inference/sparse_engine.py:224-258, with the areas of :227-228), bit for bit:
+ *   counts_dev[0] = #pixels with (double)conf_from < THRESHOLD_AREA (0.02, compared in fp64: float32(0.02) lies below
+ *   0.02), counts_dev[1] the same for conf_to; NaN is not counted.  int64, deterministic (integer atomics).
+ *   loc_to_dev[i] = (double(flow[r, c]) * 0.5 + 0.5) * (w_to, h_to), fp64 without contraction, where
+ *   r = (int)clip(y_i, 0, h_from - 1), c = (int)clip(x_i, 0, w_from - 1) with the clip in the keypoint's dtype
+ *   (sparse_engine.py:255-257, :232-234).
+ * flow_dev: h_from x w_from x 2 fp32 [-1,1] prediction in the "to" image; conf_from_dev: h_from x w_from fp32;
+ * conf_to_dev: h_to x w_to fp32 (what cotr_flow_tile_merge leaves for the two images of the pass).  kpts_dev: n x 2
+ * (x, y), float32 when kpt_is_f32 else float64, finite (the caller refuses others).  loc_to_dev: n x 2 fp64.  All DEVICE.
+ * Sizes 1 .. 65536.  Every argument is checked before anything is enqueued; one memset and one kernel, no wait.
+ * `device` is the CUDA device index. */
+int cotr_dense_first_guess(int device, const float* flow_dev, const float* conf_from_dev, int h_from, int w_from, const float* conf_to_dev,
+                           int h_to, int w_to, const void* kpts_dev, int kpt_is_f32, int n, double* loc_to_dev, int64_t* counts_dev,
+                           void* cuda_stream);
+
 /* Squad formation of the grouped scheduler (FasterSparseEngine.form_grouped_batch / form_squad,
  * COTR/inference/sparse_engine.py:295-369) on the device.  pts_dev: n x 4 fp64 [x_from, y_from, x_to, y_to] of the open
  * tasks of one zoom level in the engine's (already shuffled) order; box_dev: n x 8 fp64, the central-half boxes
@@ -325,7 +341,8 @@ int cotr_last_launch_count(const cotr_model* m);
  * 6 query_encode, 7 stem_canvas, 8 gemm_mlp (fused feed-forward block), 9 attention_weights_tc, 10 attention_weights_simt
  * (the maps of cotr_*_attention), 11 match_queries, 12 match_pixels, 13 nearest, 14 mutual (cotr_match_keypoints),
  * 15 refine_geometry, 16 resize_h, 17 resize_v, 18 refine_step (cotr_refine and cotr_refine_grouped),
- * 19 grouped_candidates, 20 group_tasks (cotr_refine_grouped).  For GEMMs M,N,K are the problem size; for attention and
+ * 19 grouped_candidates, 20 group_tasks (cotr_refine_grouped), 21 dense_first_guess (reserved: cotr_dense_first_guess
+ * takes no model, so its launch has no profiler to record it).  For GEMMs M,N,K are the problem size; for attention and
  * attention weights M = query rows, N = 512, K = 256; for 11-13 M = rows, N = 2; for 14 M = pairs; for 15 and 18
  * M = tasks of the launch (cotr_refine_grouped: its candidates), N = level; for 16-17 M = crops; for 19-20
  * M = candidates, N = level. */
