@@ -12,7 +12,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB_DIR = os.path.join(HERE, "lib")
 LIB_PATH = os.path.join(LIB_DIR, "libcotr_b200.so")
-SOURCES = ["model.cu", "gemm_simt.cu", "gemm_tc.cu", "mlp_tc.cu", "attention_simt.cu", "attention_tc.cu", "attention_weights.cu", "elementwise.cu", "preprocess.cu", "dense_post.cu", "engine_ops.cu", "peer_exchange.cu", "match.cu", "refine.cu", "first_guess.cu"]
+SOURCES = ["model.cu", "gemm_simt.cu", "gemm_tc.cu", "mlp_tc.cu", "attention_simt.cu", "attention_tc.cu", "attention_weights.cu", "elementwise.cu", "preprocess.cu", "dense_post.cu", "engine_ops.cu", "peer_exchange.cu", "match.cu", "refine.cu", "first_guess.cu", "resize.cu"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "-Xptxas", "-v"]
 

@@ -51,7 +51,8 @@ class LaunchRecord(ctypes.Structure):
 
 KERNEL_NAMES = ("gemm_tc", "gemm_simt", "attention_tc", "attention_simt", "layernorm", "maxpool", "query_encode", "stem_canvas", "gemm_mlp",
                 "attention_weights_tc", "attention_weights_simt", "match_queries", "match_pixels", "nearest", "mutual",
-                "refine_geometry", "resize_h", "resize_v", "refine_step", "grouped_candidates", "group_tasks", "dense_first_guess")
+                "refine_geometry", "resize_h", "resize_v", "refine_step", "grouped_candidates", "group_tasks", "dense_first_guess",
+                "resize_image", "resize_maps")
 
 # name -> (restype, argtypes); every symbol include/cotr_b200.h declares
 _PROTOTYPES = {
@@ -94,6 +95,13 @@ _PROTOTYPES = {
     "cotr_dense_first_guess": (ctypes.c_int, [ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_void_p,
                                               ctypes.c_int, ctypes.c_int, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_void_p,
                                               ctypes.c_void_p, ctypes.c_void_p]),
+    "cotr_dense_first_guess_f32": (ctypes.c_int, [ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_void_p,
+                                                  ctypes.c_int, ctypes.c_int, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_void_p,
+                                                  ctypes.c_void_p, ctypes.c_void_p]),
+    "cotr_resize_image": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_void_p, ctypes.c_int,
+                                         ctypes.c_int, ctypes.c_void_p]),
+    "cotr_resize_maps": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_void_p,
+                                        ctypes.c_int, ctypes.c_int, ctypes.c_void_p]),
     "cotr_rasterize_triangles": (ctypes.c_int, [ctypes.c_int, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p]),
     "cotr_exchange_create": (ctypes.c_int, [ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_size_t, ctypes.c_int, ctypes.POINTER(ctypes.c_void_p)]),
     "cotr_exchange_handle": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p]),
@@ -368,6 +376,26 @@ class NativeModel:
                                          int(patch.x), int(patch.y), int(patch.w), int(patch.h), int(patch.ow), int(patch.oh),
                                          _ptr(flow), _ptr(conf), int(bool(first)), self._stream()), "cotr_flow_tile_merge")
 
+    def resize_image(self, img, size):
+        """(H,W,3) uint8 CUDA image -> (H',W',3) uint8, Pillow's bilinear resize to size = (H',W') (cotr_resize_image)."""
+        assert img.is_cuda and img.dtype == torch.uint8 and img.ndim == 3 and img.shape[2] == 3
+        img = img.contiguous()
+        out = torch.empty((int(size[0]), int(size[1]), 3), dtype=torch.uint8, device=img.device)
+        check(lib().cotr_resize_image(self.handle, _ptr(img), img.shape[0], img.shape[1], _ptr(out), out.shape[0], out.shape[1],
+                                      self._stream()), "cotr_resize_image")
+        return out
+
+    def resize_maps(self, maps, size):
+        """(H,W) or (H,W,C) fp32 CUDA maps, C = 1 .. 3 -> the same layout at size = (H',W'), bit for bit
+        utils.float_image_resize (cotr_resize_maps)."""
+        assert maps.is_cuda and maps.dtype == torch.float32 and maps.ndim in (2, 3)
+        src = maps.contiguous()
+        c = src.shape[2] if src.ndim == 3 else 1
+        out = torch.empty((int(size[0]), int(size[1])) + tuple(src.shape[2:]), dtype=torch.float32, device=src.device)
+        check(lib().cotr_resize_maps(self.handle, _ptr(src), src.shape[0], src.shape[1], c, _ptr(out), out.shape[0], out.shape[1],
+                                     self._stream()), "cotr_resize_maps")
+        return out
+
     def set_graph_mode(self, enabled):
         check(lib().cotr_set_graph_mode(self.handle, int(bool(enabled))), "cotr_set_graph_mode")
 
@@ -521,10 +549,11 @@ def mutual_nearest(kpts, kpt_offsets, pairs, corr):
     return nearest, match, count
 
 
-def dense_first_guess(flow, conf_from, conf_to, kpts, loc_to, counts):
+def dense_first_guess(flow, conf_from, conf_to, kpts, loc_to, counts, f32_maps=False):
     """The forced first guesses of one direction (cotr_dense_first_guess).  flow (H_f,W_f,2) / conf_from (H_f,W_f) /
     conf_to (H_t,W_t): contiguous fp32 CUDA maps; kpts (n,2) float32 or float64 CUDA (x, y); outputs written in place:
-    loc_to (n,2) fp64, counts (2,) int64 (pixels below THRESHOLD_AREA in conf_from, conf_to)."""
+    loc_to (n,2) fp64, counts (2,) int64 (pixels below THRESHOLD_AREA in conf_from, conf_to).  f32_maps: the arithmetic
+    numpy does on float32 maps, as 'stretching' mode holds them (cotr_dense_first_guess_f32)."""
     for t in (flow, conf_from, conf_to, kpts, loc_to, counts):
         assert t.is_cuda and t.is_contiguous() and t.device == flow.device
     assert flow.dtype == conf_from.dtype == conf_to.dtype == torch.float32 and kpts.dtype in (torch.float32, torch.float64)
@@ -534,9 +563,9 @@ def dense_first_guess(flow, conf_from, conf_to, kpts, loc_to, counts):
     assert counts.dtype == torch.int64 and counts.shape == (2,)
     dev = flow.device.index if flow.device.index is not None else torch.cuda.current_device()
     stream = ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
-    check(lib().cotr_dense_first_guess(dev, _ptr(flow), _ptr(conf_from), flow.shape[0], flow.shape[1], _ptr(conf_to), conf_to.shape[0],
-                                       conf_to.shape[1], _ptr(kpts), int(kpts.dtype == torch.float32), n, _ptr(loc_to), _ptr(counts),
-                                       stream), "cotr_dense_first_guess")
+    name = "cotr_dense_first_guess_f32" if f32_maps else "cotr_dense_first_guess"
+    check(getattr(lib(), name)(dev, _ptr(flow), _ptr(conf_from), flow.shape[0], flow.shape[1], _ptr(conf_to), conf_to.shape[0],
+                               conf_to.shape[1], _ptr(kpts), int(kpts.dtype == torch.float32), n, _ptr(loc_to), _ptr(counts), stream), name)
 
 
 def rasterize_triangles(tris, H, W):

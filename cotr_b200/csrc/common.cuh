@@ -5,6 +5,7 @@
 #include <cstdarg>
 #include <cstdint>
 #include <cstdio>
+#include <vector>
 
 namespace cotr {
 
@@ -366,6 +367,32 @@ int preprocess_coeffs(Preprocessor* p, int size, CropSide* side);
 // The two resize passes over n_sides prepared sides (device table) of side length <= max_size.
 int launch_resize_h(const CropSide* sides, int n_sides, int max_size, unsigned char* tmp, cudaStream_t s);
 int launch_resize_v(const CropSide* sides, int n_sides, const unsigned char* tmp, float* canvas, cudaStream_t s);
+
+// Pillow's bilinear coefficient tables for an in_size -> out_size axis: 22-bit fixed point for 8-bit images
+// (preprocess.cu) and double for mode 'F' (engine_ops.cu).  bounds: out_size x [first source index, tap count].
+void host_coeffs(int in_size, int out_size, std::vector<int>& bounds, std::vector<int>& weights, int& ksize);
+void host_float_coeffs(int in_size, int out_size, std::vector<int>& bounds, std::vector<double>& weights, int& ksize);
+
+// Whole-image Pillow-exact resizes of cotr_resize_image / cotr_resize_maps (resize.cu).  resize_plan checks nothing (the
+// C ABI does), fetches or builds the two axes' tables and grows the intermediate buffer; resize_pass enqueues one pass.
+struct Resizer;
+Resizer* resizer_create();
+void resizer_destroy(Resizer* r);
+struct ResizeAxis {
+    int ksize = 0;
+    const int* bounds = nullptr;
+    const void* weights = nullptr;   // int (8-bit images) or double (float maps)
+};
+struct ResizePlan {
+    int u8;                     // 1: uint8 HWC, c = 3; 0: fp32 HWC, c = 1 .. 3
+    int h, w, c, oh, ow;
+    int need_h, need_v;         // Pillow skips an axis whose size does not change
+    ResizeAxis horiz, vert;
+    void* tmp;                  // h x ow x c intermediate of the horizontal pass (when both passes run)
+};
+int resize_plan(Resizer* r, int u8, int h, int w, int c, int oh, int ow, ResizePlan* p);
+// pass 0: horizontal, (h, w) -> (h, ow); pass 1: vertical, (h, ow) -> (oh, ow)
+int resize_pass(const ResizePlan& p, int pass, const void* src, void* dst, cudaStream_t s);
 
 // Zoom-in walks of cotr_refine and cotr_refine_grouped (refine.cu).  One level: the crops of `count` entries at one zoom
 // level, entry i being task task0 + ids[i].

@@ -80,14 +80,7 @@ int rasterize_triangles_launch(const float* tris, int n_tri, int H, int W, float
 // coefficients (precompute_coeffs), double accumulation `ss += pixel * k` with separate multiply and add (the x86-64
 // build has no FMA contraction: __dmul_rn / __dadd_rn), float32 store after each of the two passes.
 // =====================================================================================================================
-namespace {
-
-struct FloatCoeffs {
-    int ksize = 0;
-    int* bounds = nullptr;      // device [out][2]
-    double* weights = nullptr;  // device [out][ksize]
-};
-
+// Shared with the map resize of cotr_resize_maps (resize.cu).
 void host_float_coeffs(int in_size, int out_size, std::vector<int>& bounds, std::vector<double>& weights, int& ksize) {
     const double scale = (double)((float)in_size - 0.0f) / out_size;
     const double filterscale = scale < 1.0 ? 1.0 : scale;
@@ -118,6 +111,14 @@ void host_float_coeffs(int in_size, int out_size, std::vector<int>& bounds, std:
         bounds[(size_t)xx * 2 + 1] = xmax;
     }
 }
+
+namespace {
+
+struct FloatCoeffs {
+    int ksize = 0;
+    int* bounds = nullptr;      // device [out][2]
+    double* weights = nullptr;  // device [out][ksize]
+};
 
 struct TileJob {
     const float* tile;        // (256, 256, 3) [x, y, confidence], row pitch `pitch` floats

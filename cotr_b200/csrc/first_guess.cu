@@ -6,6 +6,10 @@
 //     NaN compares false.  Integer atomics: the counts do not depend on the schedule.
 //   * per keypoint the dense prediction at the clipped, truncated pixel, mapped to pixels of the other image:
 //     (double(flow) * 0.5 + 0.5) * (W_to, H_to) with separate multiply and add (no contraction).
+// cotr_dense_first_guess_f32 is the same branch on float32 maps, which is what 'stretching' mode hands gen_tasks when
+// an image had to be stretched (float_image_resize returns float32): numpy then compares `conf < 0.02` in float32, so
+// float32(0.02) itself is not counted, and computes `corr * 0.5 + 0.5` in float32 before the multiply by the int64
+// image size widens it to fp64.
 #include <algorithm>
 
 #include "../../include/cotr_b200.h"
@@ -15,6 +19,7 @@ namespace cotr {
 namespace {
 
 constexpr double kThresholdArea = 0.02;   // inference_helper.THRESHOLD_AREA
+constexpr float kThresholdAreaF32 = 0.02f;
 constexpr int kThreads = 256;
 
 struct FirstGuessArgs {
@@ -24,6 +29,7 @@ struct FirstGuessArgs {
     const void* kpts;           // (n, 2) float32 or float64 (x, y)
     int64_t px_from, px_to;
     int h_from, w_from, h_to, w_to, n, f32;
+    int f32_maps;               // float32 semantics of the maps (cotr_dense_first_guess_f32)
     double* loc_to;             // (n, 2)
     unsigned long long* counts; // [from, to], zeroed before the launch
 };
@@ -44,12 +50,22 @@ __global__ void __launch_bounds__(kThreads) dense_first_guess_kernel(const First
             c = (int)fmin(fmax(k[0], 0.0), (double)(a.w_from - 1));
         }
         const float* f = a.flow + ((int64_t)r * a.w_from + c) * 2;
-        a.loc_to[2 * i] = __dmul_rn(__dadd_rn(__dmul_rn((double)f[0], 0.5), 0.5), (double)a.w_to);
-        a.loc_to[2 * i + 1] = __dmul_rn(__dadd_rn(__dmul_rn((double)f[1], 0.5), 0.5), (double)a.h_to);
+        if (a.f32_maps) {
+            a.loc_to[2 * i] = __dmul_rn((double)__fadd_rn(__fmul_rn(f[0], 0.5f), 0.5f), (double)a.w_to);
+            a.loc_to[2 * i + 1] = __dmul_rn((double)__fadd_rn(__fmul_rn(f[1], 0.5f), 0.5f), (double)a.h_to);
+        } else {
+            a.loc_to[2 * i] = __dmul_rn(__dadd_rn(__dmul_rn((double)f[0], 0.5), 0.5), (double)a.w_to);
+            a.loc_to[2 * i + 1] = __dmul_rn(__dadd_rn(__dmul_rn((double)f[1], 0.5), 0.5), (double)a.h_to);
+        }
     }
     unsigned int below_from = 0, below_to = 0;      // at most ceil(65536^2 / (132 * 8 * 256)) per thread
-    for (int64_t p = tid; p < a.px_from; p += stride) below_from += (double)a.conf_from[p] < kThresholdArea ? 1u : 0u;
-    for (int64_t p = tid; p < a.px_to; p += stride) below_to += (double)a.conf_to[p] < kThresholdArea ? 1u : 0u;
+    if (a.f32_maps) {
+        for (int64_t p = tid; p < a.px_from; p += stride) below_from += a.conf_from[p] < kThresholdAreaF32 ? 1u : 0u;
+        for (int64_t p = tid; p < a.px_to; p += stride) below_to += a.conf_to[p] < kThresholdAreaF32 ? 1u : 0u;
+    } else {
+        for (int64_t p = tid; p < a.px_from; p += stride) below_from += (double)a.conf_from[p] < kThresholdArea ? 1u : 0u;
+        for (int64_t p = tid; p < a.px_to; p += stride) below_to += (double)a.conf_to[p] < kThresholdArea ? 1u : 0u;
+    }
     below_from = __reduce_add_sync(0xffffffffu, below_from);
     below_to = __reduce_add_sync(0xffffffffu, below_to);
     if ((threadIdx.x & 31) == 0) {
@@ -58,14 +74,9 @@ __global__ void __launch_bounds__(kThreads) dense_first_guess_kernel(const First
     }
 }
 
-}  // namespace
-}  // namespace cotr
-
-int cotr_dense_first_guess(int device, const float* flow_dev, const float* conf_from_dev, int h_from, int w_from, const float* conf_to_dev,
-                           int h_to, int w_to, const void* kpts_dev, int kpt_is_f32, int n, double* loc_to_dev, int64_t* counts_dev,
-                           void* cuda_stream) {
-    using namespace cotr;
-    const char* fn = "cotr_dense_first_guess";
+int first_guess_impl(const char* fn, int f32_maps, int device, const float* flow_dev, const float* conf_from_dev, int h_from, int w_from,
+                     const float* conf_to_dev, int h_to, int w_to, const void* kpts_dev, int kpt_is_f32, int n, double* loc_to_dev,
+                     int64_t* counts_dev, void* cuda_stream) {
     COTR_CHECK(h_from >= 1 && w_from >= 1 && h_to >= 1 && w_to >= 1 && h_from <= 65536 && w_from <= 65536 && h_to <= 65536 && w_to <= 65536,
                "%s: image sizes %d x %d and %d x %d must lie in 1 .. 65536", fn, h_from, w_from, h_to, w_to);
     COTR_CHECK(n >= 0, "%s: n = %d keypoints", fn, n);
@@ -82,6 +93,7 @@ int cotr_dense_first_guess(int device, const float* flow_dev, const float* conf_
     a.flow = flow_dev; a.conf_from = conf_from_dev; a.conf_to = conf_to_dev; a.kpts = kpts_dev;
     a.px_from = (int64_t)h_from * w_from; a.px_to = (int64_t)h_to * w_to;
     a.h_from = h_from; a.w_from = w_from; a.h_to = h_to; a.w_to = w_to; a.n = n; a.f32 = kpt_is_f32;
+    a.f32_maps = f32_maps;
     a.loc_to = loc_to_dev;
     a.counts = reinterpret_cast<unsigned long long*>(counts_dev);
     const int64_t work = std::max<int64_t>(std::max(a.px_from, a.px_to), n);
@@ -90,4 +102,21 @@ int cotr_dense_first_guess(int device, const float* flow_dev, const float* conf_
     dense_first_guess_kernel<<<grid, kThreads, 0, s>>>(a);
     COTR_CHECK_CUDA(cudaGetLastError());
     return 0;
+}
+
+}  // namespace
+}  // namespace cotr
+
+int cotr_dense_first_guess(int device, const float* flow_dev, const float* conf_from_dev, int h_from, int w_from, const float* conf_to_dev,
+                           int h_to, int w_to, const void* kpts_dev, int kpt_is_f32, int n, double* loc_to_dev, int64_t* counts_dev,
+                           void* cuda_stream) {
+    return cotr::first_guess_impl("cotr_dense_first_guess", 0, device, flow_dev, conf_from_dev, h_from, w_from, conf_to_dev, h_to, w_to,
+                                  kpts_dev, kpt_is_f32, n, loc_to_dev, counts_dev, cuda_stream);
+}
+
+int cotr_dense_first_guess_f32(int device, const float* flow_dev, const float* conf_from_dev, int h_from, int w_from,
+                               const float* conf_to_dev, int h_to, int w_to, const void* kpts_dev, int kpt_is_f32, int n, double* loc_to_dev,
+                               int64_t* counts_dev, void* cuda_stream) {
+    return cotr::first_guess_impl("cotr_dense_first_guess_f32", 1, device, flow_dev, conf_from_dev, h_from, w_from, conf_to_dev, h_to, w_to,
+                                  kpts_dev, kpt_is_f32, n, loc_to_dev, counts_dev, cuda_stream);
 }

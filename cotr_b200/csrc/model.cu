@@ -201,6 +201,7 @@ struct cotr_model {
     cotr::PinnedTable<int32_t> grouped_ids;   // cotr_refine_grouped: the batch's permuted candidate task ids
     cotr::Preprocessor* pre = nullptr;         // device-side crop / resize / normalise (cotr_preprocess)
     cotr::FlowMerger* merger = nullptr;        // device-side tail of the dense first guess (cotr_flow_tile_merge)
+    cotr::Resizer* resizer = nullptr;          // whole-image resizes (cotr_resize_image, cotr_resize_maps)
     bool prof_on = false;
     std::vector<cudaEvent_t> prof_events;      // 2 per record
     std::vector<cotr_launch_record> prof_records;
@@ -385,7 +386,7 @@ struct Run {
 enum KernelId { K_GEMM_TC = 0, K_GEMM_SIMT = 1, K_ATTN_TC = 2, K_ATTN_SIMT = 3, K_LAYERNORM = 4, K_MAXPOOL = 5, K_QENC = 6, K_STEM_CANVAS = 7,
                 K_GEMM_MLP = 8, K_ATTN_WEIGHTS_TC = 9, K_ATTN_WEIGHTS_SIMT = 10, K_MATCH_QUERIES = 11, K_MATCH_PIXELS = 12,
                 K_NEAREST = 13, K_MUTUAL = 14, K_REFINE_GEOMETRY = 15, K_RESIZE_H = 16, K_RESIZE_V = 17, K_REFINE_STEP = 18,
-                K_GROUPED_CANDIDATES = 19, K_GROUP_TASKS = 20, K_DENSE_FIRST_GUESS = 21 };
+                K_GROUPED_CANDIDATES = 19, K_GROUP_TASKS = 20, K_DENSE_FIRST_GUESS = 21, K_RESIZE_IMAGE = 22, K_RESIZE_MAPS = 23 };
 
 // Counts the launch and, when the profiler is on, brackets it with two events on the launching stream.
 struct LaunchScope {
@@ -1528,6 +1529,7 @@ void cotr_destroy(cotr_model* m) {
     for (auto& kv : m->graphs) cudaGraphExecDestroy(kv.second);
     preprocessor_destroy(m->pre);
     flow_merger_destroy(m->merger);
+    resizer_destroy(m->resizer);
     for (cudaEvent_t e : m->prof_events) cudaEventDestroy(e);
     if (m->order_event) cudaEventDestroy(m->order_event);
     delete m;
@@ -2122,6 +2124,49 @@ int cotr_flow_tile_merge(cotr_model* m, const float* tile_dev, int pitch_floats,
     CallOrder order(m, (cudaStream_t)cuda_stream);
     return flow_tile_merge_launch(m->merger, tile_dev, pitch_floats, affine_host, px, py, pw, ph, ow, oh, flow_dev, conf_dev, first,
                                   (cudaStream_t)cuda_stream);
+}
+
+// cotr_resize_image and cotr_resize_maps: every argument checked, then at most two passes (or one copy) on the stream.
+static int resize_impl(cotr_model* m, const char* fn, int u8, const void* src, int h, int w, int c, void* dst, int out_h, int out_w,
+                       void* cuda_stream) {
+    COTR_CHECK(m != nullptr, "%s: null model", fn);
+    COTR_CHECK(src && dst, "%s: null src_dev or dst_dev", fn);
+    COTR_CHECK(h >= 1 && w >= 1 && out_h >= 1 && out_w >= 1 && h <= 65536 && w <= 65536 && out_h <= 65536 && out_w <= 65536,
+               "%s: sizes %d x %d -> %d x %d must lie in 1 .. 65536", fn, h, w, out_h, out_w);
+    COTR_CHECK(c >= 1 && c <= 3, "%s: %d channels (1 .. 3)", fn, c);
+    const size_t elem = u8 ? 1 : sizeof(float);
+    COTR_CHECK(u8 || (((uintptr_t)src & 3) == 0 && ((uintptr_t)dst & 3) == 0), "%s: src_dev or dst_dev is not 4-byte aligned", fn);
+    const uintptr_t s0 = (uintptr_t)src, s1 = s0 + (size_t)h * w * c * elem, d0 = (uintptr_t)dst, d1 = d0 + (size_t)out_h * out_w * c * elem;
+    COTR_CHECK(d1 <= s0 || s1 <= d0, "%s: src_dev and dst_dev overlap", fn);
+    COTR_CHECK_CUDA(cudaSetDevice(m->device));
+    if (!m->resizer) m->resizer = resizer_create();
+    cudaStream_t s = (cudaStream_t)cuda_stream;
+    ResizePlan p;
+    if (resize_plan(m->resizer, u8, h, w, c, out_h, out_w, &p)) return 1;
+    CallOrder order(m, s);
+    const Run r{m, s};
+    const int kernel = u8 ? K_RESIZE_IMAGE : K_RESIZE_MAPS;
+    if (!p.need_h && !p.need_v) {
+        COTR_CHECK_CUDA(cudaMemcpyAsync(dst, src, (size_t)h * w * c * elem, cudaMemcpyDeviceToDevice, s));
+        return 0;
+    }
+    if (p.need_h) {
+        LaunchScope ls(r, kernel, h, out_w, 0);
+        if (resize_pass(p, 0, src, p.need_v ? p.tmp : dst, s)) return 1;
+    }
+    if (p.need_v) {
+        LaunchScope ls(r, kernel, out_h, out_w, 1);
+        if (resize_pass(p, 1, p.need_h ? p.tmp : src, dst, s)) return 1;
+    }
+    return 0;
+}
+
+int cotr_resize_image(cotr_model* m, const uint8_t* src_dev, int h, int w, uint8_t* dst_dev, int out_h, int out_w, void* cuda_stream) {
+    return resize_impl(m, "cotr_resize_image", 1, src_dev, h, w, 3, dst_dev, out_h, out_w, cuda_stream);
+}
+
+int cotr_resize_maps(cotr_model* m, const float* src_dev, int h, int w, int c, float* dst_dev, int out_h, int out_w, void* cuda_stream) {
+    return resize_impl(m, "cotr_resize_maps", 0, src_dev, h, w, c, dst_dev, out_h, out_w, cuda_stream);
 }
 
 int cotr_group_tasks(int device, const double* pts_dev, const double* box_dev, int n, int batch_size, int max_load, int32_t* squad_dev,

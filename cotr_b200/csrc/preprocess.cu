@@ -24,18 +24,21 @@ struct CoeffTable {
     int* weights = nullptr;   // device [256][ksize]
 };
 
-// libImaging/Resample.c precompute_coeffs + normalize_coeffs_8bpc for the bilinear filter (support 1.0), box = whole
-// crop.  Plain double arithmetic on the host (no FMA contraction on x86-64 baseline), so the integers match Pillow's.
-void host_coeffs(int in_size, std::vector<int>& bounds, std::vector<int>& weights, int& ksize) {
-    const double scale = (double)((float)in_size - 0.0f) / kOut;
+}  // namespace
+
+// libImaging/Resample.c precompute_coeffs + normalize_coeffs_8bpc for the bilinear filter (support 1.0), box = the whole
+// input, any output size.  Plain double arithmetic on the host (no FMA contraction on x86-64 baseline), so the integers
+// match Pillow's.  Shared with the image resize of cotr_resize_image (resize.cu).
+void host_coeffs(int in_size, int out_size, std::vector<int>& bounds, std::vector<int>& weights, int& ksize) {
+    const double scale = (double)((float)in_size - 0.0f) / out_size;
     const double filterscale = scale < 1.0 ? 1.0 : scale;
     const double support = 1.0 * filterscale;
     ksize = (int)std::ceil(support) * 2 + 1;
-    bounds.assign(kOut * 2, 0);
-    weights.assign((size_t)kOut * ksize, 0);
+    bounds.assign((size_t)out_size * 2, 0);
+    weights.assign((size_t)out_size * ksize, 0);
     std::vector<double> k(ksize);
     const double ss = 1.0 / filterscale;
-    for (int xx = 0; xx < kOut; ++xx) {
+    for (int xx = 0; xx < out_size; ++xx) {
         const double center = 0.0 + (xx + 0.5) * scale;
         double ww = 0.0;
         int xmin = (int)(center - support + 0.5);
@@ -56,10 +59,12 @@ void host_coeffs(int in_size, std::vector<int>& bounds, std::vector<int>& weight
             const double v = x < xmax ? k[x] : 0.0;
             weights[(size_t)xx * ksize + x] = v < 0 ? (int)(-0.5 + v * (1 << kPrecisionBits)) : (int)(0.5 + v * (1 << kPrecisionBits));
         }
-        bounds[xx * 2] = xmin;
-        bounds[xx * 2 + 1] = xmax;
+        bounds[(size_t)xx * 2] = xmin;
+        bounds[(size_t)xx * 2 + 1] = xmax;
     }
 }
+
+namespace {
 
 __device__ __forceinline__ unsigned char clip8(int v) {
     v >>= kPrecisionBits;
@@ -149,7 +154,7 @@ static int get_table(Preprocessor* p, int size, CoeffTable* out) {
     if (it == p->tables.end()) {
         std::vector<int> b, w;
         CoeffTable t;
-        host_coeffs(size, b, w, t.ksize);
+        host_coeffs(size, kOut, b, w, t.ksize);
         COTR_CHECK_CUDA(cudaMalloc((void**)&t.bounds, b.size() * sizeof(int)));
         COTR_CHECK_CUDA(cudaMalloc((void**)&t.weights, w.size() * sizeof(int)));
         COTR_CHECK_CUDA(cudaMemcpy(t.bounds, b.data(), b.size() * sizeof(int), cudaMemcpyHostToDevice));

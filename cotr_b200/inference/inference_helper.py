@@ -22,6 +22,7 @@ THRESHOLD_PIXELS_RELATIVE = 0.02
 BASE_ZOOM = 1.0
 DEVICE_DENSE_POST = True   # native model: finish the dense pass on the device (cotr_dense_postprocess); False = host path
 DEVICE_FLOW_MERGE = True   # native model: patch affine + float_image_resize + tile merge on the device (cotr_flow_tile_merge)
+DEVICE_STRETCH = True      # native model: 'stretching' mode stretches, dense-passes and resizes back on the device
 THRESHOLD_AREA = 0.02
 LARGE_GPU = True
 
@@ -228,18 +229,46 @@ def _device_pixels(img):
     return isinstance(img, np.ndarray) and img.dtype == np.uint8 and img.ndim == 3 and img.shape[2] == 3
 
 
-def cotr_flow(model, img_a, img_b):
-    """Dense correspondence maps in [-1,1] + cycle confidence + warped images, both directions (:168-182)."""
-    patches_a, patches_b = to_square_patches(img_a), to_square_patches(img_b)
-    if (LARGE_GPU and DEVICE_DENSE_POST and DEVICE_FLOW_MERGE and hasattr(model, 'flow_tile_merge') and hasattr(model, 'dense_postprocess')
+def flow_on_device(model, img_a, img_b):
+    """Whether cotr_flow's maps come from the device path (dense_flow_maps) for this model and these images."""
+    return (LARGE_GPU and DEVICE_DENSE_POST and DEVICE_FLOW_MERGE and hasattr(model, 'flow_tile_merge') and hasattr(model, 'dense_postprocess')
             and hasattr(model, 'preprocess_canvases') and _device_pixels(img_a) and _device_pixels(img_b)
-            and _model_device(model).type == 'cuda'):
+            and _model_device(model).type == 'cuda')
+
+
+def cotr_flow_maps(model, img_a, img_b):
+    """The maps of cotr_flow without the two warped images: (corr_a, con_a, corr_b, con_b), float64."""
+    patches_a, patches_b = to_square_patches(img_a), to_square_patches(img_b)
+    if flow_on_device(model, img_a, img_b):
         (corr_a, con_a), (corr_b, con_b) = _cotr_flow_device(model, img_a, img_b, patches_a, patches_b)
     else:
         corrs_a, corrs_b = cotr_patch_flow_exhaustive(model, patches_a, patches_b)
         corr_a, con_a, _ = merge_flow_patches(corrs_a)
         corr_b, con_b, _ = merge_flow_patches(corrs_b)
+    return corr_a, con_a, corr_b, con_b
+
+
+def cotr_flow(model, img_a, img_b):
+    """Dense correspondence maps in [-1,1] + cycle confidence + warped images, both directions (:168-182)."""
+    corr_a, con_a, corr_b, con_b = cotr_flow_maps(model, img_a, img_b)
     return corr_a, con_a, _resample(img_b, corr_a), corr_b, con_b, _resample(img_a, corr_b)
+
+
+def stretch_to_square(model, img_dev):
+    """A uint8 HWC CUDA image resized to max(h, w) squared on the device, bit for bit sparse_engine.stretch_to_square_np
+    (a square image is returned as it is: Pillow would copy it)."""
+    h, w = int(img_dev.shape[0]), int(img_dev.shape[1])
+    return img_dev if h == w else model.resize_image(img_dev, (max(h, w), max(h, w)))
+
+
+def stretched_flow_maps(model, img_a_dev, img_b_dev, shape_a, shape_b):
+    """'stretching' mode's dense first guess on the device: both uint8 CUDA images stretched to max(h, w) squares
+    (COTR.resize_image, bit for bit stretch_to_square_np), one dense pass on the squares (each is a single tile), and the
+    flow and confidence maps resized back to the original (H, W) shapes (COTR.resize_maps, bit for bit
+    utils.float_image_resize) -> ((flow_a (H_a,W_a,2), conf_a (H_a,W_a)), (flow_b, conf_b)) fp32 CUDA tensors."""
+    sq_a, sq_b = stretch_to_square(model, img_a_dev), stretch_to_square(model, img_b_dev)
+    maps = dense_flow_maps(model, sq_a, sq_b, to_square_patches(sq_a), to_square_patches(sq_b))
+    return tuple((model.resize_maps(flow, shape), model.resize_maps(conf, shape)) for (flow, conf), shape in zip(maps, (shape_a, shape_b)))
 
 
 def _sparse_pass(model, img_a, img_b, queries):

@@ -11,7 +11,7 @@ import torch
 
 from .. import capi
 from . import refinement_task
-from .inference_helper import dense_flow_maps, get_patch_centered_at, to_square_patches
+from .inference_helper import dense_flow_maps, get_patch_centered_at, stretch_to_square, to_square_patches
 from .refinement_task import crop_scales
 from .sparse_engine import _exact_point
 
@@ -61,17 +61,18 @@ def _check_keypoints(keypoints, n_images):
     return out
 
 
-def _check_images(images):
-    """-> the (H, W) of every image; uint8 HWC RGB arrays or tensors, long side <= 2 x short side (to_square_patches)."""
+def _check_images(images, tiled=True):
+    """-> the (H, W) of every image; uint8 HWC RGB arrays or tensors, and when `tiled` (mode 'tile') long side <= 2 x
+    short side (to_square_patches)."""
     shapes = []
     for i, img in enumerate(images):
         ok = img.dtype == torch.uint8 if isinstance(img, torch.Tensor) else isinstance(img, np.ndarray) and img.dtype == np.uint8
         if not (ok and img.ndim == 3 and img.shape[2] == 3):
             raise ValueError(f"images: image {i} must be a uint8 H x W x 3 array or tensor, got {tuple(img.shape)} {img.dtype}")
         h, w = int(img.shape[0]), int(img.shape[1])
-        if max(h, w) > 2 * min(h, w):
+        if tiled and max(h, w) > 2 * min(h, w):
             raise NotImplementedError(f"images: image {i} is {h} x {w}; the dense pass tiles images whose long side is at most "
-                                      "twice the short side (to_square_patches)")
+                                      "twice the short side (to_square_patches); mode='stretching' takes any shape")
         shapes.append((h, w))
     return shapes
 
@@ -130,33 +131,40 @@ def check_crops(groups, scales, shapes, zooms, first_guesses=None):
 
 
 @torch.no_grad()
-def match_keypoints_multiscale(model, images, keypoints, pairs, zoom_ins=np.linspace(0.5, 0.0625, 4), batch_size=32):
+def match_keypoints_multiscale(model, images, keypoints, pairs, zoom_ins=np.linspace(0.5, 0.0625, 4), batch_size=32, mode='tile'):
     """Mutual nearest-neighbour matches of keypoints across image pairs through the whole zoom-in of
     demo_guided_matching.py, on the device.  For pair p = (a, b) the results equal, bit for bit,
 
-        eng = SparseEngine(model, batch_size, mode='tile', device_walk=True)
+        eng = SparseEngine(model, batch_size, mode=mode, device_walk=True)
         c_ab = eng.cotr_corr_multiscale(img_a, img_b, zoom_ins, 1, max_corrs=len(kp_a), queries_a=kp_a, force=True)
         c_ba = eng.cotr_corr_multiscale(img_b, img_a, zoom_ins, 1, max_corrs=len(kp_b), queries_a=kp_b, force=True)
         mutual_nearest(c_ab[:, 2:], kp_b, c_ba[:, 2:], kp_a)
 
-    images: N uint8 H x W x 3 RGB arrays or CUDA tensors (sizes may differ; long side <= 2 x short side);
+    mode: the engine's first-guess mode.  'tile' (the default) runs the dense pass on each image's square tiles and takes
+    images whose long side is at most twice the short side.  'stretching' runs it once per direction on both images
+    stretched to max(h, w) squares on the device, resizes the maps back to the images' shapes, and takes any shape; when
+    an image of the pair is not square the first guesses and area counts then follow the engine's float32 arithmetic on
+    the resized maps (cotr_dense_first_guess_f32).  The crops of the walk are always cut from the original images.
+    images: N uint8 H x W x 3 RGB arrays or CUDA tensors (sizes may differ);
     keypoints: N (K_i,2) float32 or float64 (x, y) pixel arrays; pairs: (B,2) image indices.  -> KeypointMatches
     (cotr_b200.models.cotr_model): matches[p] (M_p,2) int64, corrs_ab[p] (K_a,2) / corrs_ba[p] (K_b,2) fp64 (c_ab[:, 2:],
     c_ba[:, 2:]), nearest_ab[p] / nearest_ba[p] int32, all device tensors.  An image without keypoints walks no
     direction from it, and its pairs get no matches.
 
-    Every direction runs the dense pass of cotr_flow on the device (one forward per tile pair) and cotr_dense_first_guess;
+    Every direction runs the dense pass of cotr_flow (or of the stretched squares) on the device and cotr_dense_first_guess;
     one small copy brings back the area counts, the crop scales are computed on the host, and one cotr_refine call
     walks every direction of every pair; cotr_mutual_nearest keeps the mutual matches and one last copy reads the B match
     counts.  Raises what the per-pair engine raises (ValueError on a NaN scale or prediction), refuses attention hooks,
     models without the native extensions and keypoints the device walk cannot take exactly."""
     from ..models.cotr_model import KeypointMatches
+    if mode not in ('tile', 'stretching'):
+        raise ValueError(f"mode must be 'tile' or 'stretching', got {mode!r}")
     zooms = [float(z) for z in zoom_ins]
     if not 1 <= len(zooms) <= 7:
         raise ValueError(f"zoom_ins: {len(zooms)} levels; the device walk takes 1 .. 7")
     if not (isinstance(batch_size, (int, np.integer)) and batch_size >= 1):
         raise ValueError(f"batch_size must be a positive integer, got {batch_size!r}")
-    shapes = _check_images(images)
+    shapes = _check_images(images, tiled=mode == 'tile')
     kps = _check_keypoints(keypoints, len(images))
     pairs = _check_pairs(pairs, len(images))
     _check_model(model)
@@ -173,12 +181,24 @@ def match_keypoints_multiscale(model, images, keypoints, pairs, zoom_ins=np.lins
     if n:
         img_dev = [img.to(dev).contiguous() if isinstance(img, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(img)).to(dev)
                    for img in images]
-        patches = [to_square_patches(img) for img in img_dev]
+        patches, squares = {}, {}                     # per image, made on first use
         loc_to = torch.empty((n, 2), dtype=torch.float64, device=dev)
         below = torch.empty((len(groups), 2), dtype=torch.int64, device=dev)
         for g, (_, f, t, first, count) in enumerate(groups):
-            (flow_f, conf_f), (_, conf_t) = dense_flow_maps(model, img_dev[f], img_dev[t], patches[f], patches[t])
-            capi.dense_first_guess(flow_f, conf_f, conf_t, kp_dev[f], loc_to[first:first + count], below[g])
+            stretch = mode == 'stretching' and any(shapes[i][0] != shapes[i][1] for i in (f, t))
+            if stretch:
+                for i in (f, t):
+                    if i not in squares:
+                        squares[i] = stretch_to_square(model, img_dev[i])
+                sq_f, sq_t = squares[f], squares[t]
+                (flow_f, conf_f), (_, conf_t) = dense_flow_maps(model, sq_f, sq_t, to_square_patches(sq_f), to_square_patches(sq_t))
+                flow_f, conf_f, conf_t = (model.resize_maps(m, shapes[i]) for m, i in ((flow_f, f), (conf_f, f), (conf_t, t)))
+            else:
+                for i in (f, t):
+                    if i not in patches:
+                        patches[i] = to_square_patches(img_dev[i])
+                (flow_f, conf_f), (_, conf_t) = dense_flow_maps(model, img_dev[f], img_dev[t], patches[f], patches[t])
+            capi.dense_first_guess(flow_f, conf_f, conf_t, kp_dev[f], loc_to[first:first + count], below[g], f32_maps=stretch)
         # one copy: the area counts and whether a first guess is not finite (a NaN / inf dense prediction)
         host = torch.cat([below.view(-1), (~torch.isfinite(loc_to)).any().view(1).long()]).cpu().numpy()
         scales = group_scales(host[:-1].reshape(-1, 2), shapes, groups)

@@ -14,7 +14,9 @@ import PIL.Image
 import torch
 
 from . import refinement_task
-from .inference_helper import THRESHOLD_SPARSE, THRESHOLD_AREA, cotr_flow, cotr_corr_base, get_patch_centered_at
+from . import inference_helper
+from .inference_helper import (THRESHOLD_SPARSE, THRESHOLD_AREA, cotr_corr_base, cotr_flow_maps, flow_on_device, get_patch_centered_at,
+                               stretched_flow_maps)
 from .refinement_task import RefinementTask
 from ..utils import utils
 from ..utils.utils import ImagePatch
@@ -105,7 +107,8 @@ class SparseEngine():
         self._dev_images = {}
 
     # ---- device-side pixels --------------------------------------------------------------------------------
-    def _use_device_pixels(self, tasks):
+    def _device_pixels_fit(self, images):
+        """The model takes pixels on the device and every image is a uint8 HWC RGB array."""
         if not (self.device_preprocess and getattr(self.model, 'supports_device_preprocess', False)):
             return False
         try:
@@ -113,11 +116,18 @@ class SparseEngine():
                 return False
         except StopIteration:
             return False
+        return all(isinstance(img, np.ndarray) and img.dtype == np.uint8 and img.ndim == 3 and img.shape[2] == 3 for img in images)
+
+    def _use_device_pixels(self, tasks):
         first = tasks[0]
-        for img in (first.image_from, first.image_to):
-            if not (isinstance(img, np.ndarray) and img.dtype == np.uint8 and img.ndim == 3 and img.shape[2] == 3):
-                return False
+        if not self._device_pixels_fit((first.image_from, first.image_to)):
+            return False
         return all(t.image_from is first.image_from and t.image_to is first.image_to for t in tasks)
+
+    def _device_stretch(self, img_a, img_b):
+        """'stretching' mode's stretch, dense pass and resize back run on the device (stretched_flow_maps)."""
+        return (inference_helper.DEVICE_STRETCH and hasattr(self.model, 'resize_image') and hasattr(self.model, 'resize_maps')
+                and self._device_pixels_fit((img_a, img_b)) and flow_on_device(self.model, img_a, img_b))
 
     def _device_image(self, img):
         key = (id(img), img.shape)
@@ -204,15 +214,25 @@ class SparseEngine():
         return [RefinementTask(img_a, img_b, c[:2], c[2:], areas[0], areas[1], converge_iters, zoom_ins) for c in corr_a]
 
     def _dense_first_guess(self, img_a, img_b):
-        """cotr_flow on the pair (stretched to squares in 'stretching' mode, :114-139)."""
+        """cotr_flow's maps on the pair (stretched to squares in 'stretching' mode, :114-139) as
+        (corr_a, con_a, None, corr_b, con_b, None): the warped images cotr_flow also returns are never used here, so they
+        are not computed.  The maps are float64, except after a stretch, where float_image_resize leaves them float32
+        (which changes gen_tasks' arithmetic: its compares and first guesses then run in float32).  With the native model
+        the stretch, the dense pass and the resize back run on the device, and only the four maps come to the host."""
         needs_stretch = self.mode == 'stretching' and (img_a.shape[0] != img_a.shape[1] or img_b.shape[0] != img_b.shape[1])
         if self.mode not in ('stretching', 'tile'):
             raise ValueError(f'unsupported mode: {self.mode}')
         if not needs_stretch:
-            return cotr_flow(self.model, img_a, img_b)
-        maps = cotr_flow(self.model, stretch_to_square_np(img_a.copy()), stretch_to_square_np(img_b.copy()))
-        shapes = (img_a.shape[:2],) * 3 + (img_b.shape[:2],) * 3
-        return tuple(utils.float_image_resize(m, s) for m, s in zip(maps, shapes))
+            corr_a, con_a, corr_b, con_b = cotr_flow_maps(self.model, img_a, img_b)
+            return corr_a, con_a, None, corr_b, con_b, None
+        shape_a, shape_b = img_a.shape[:2], img_b.shape[:2]
+        if self._device_stretch(img_a, img_b):
+            (corr_a, con_a), (corr_b, con_b) = stretched_flow_maps(self.model, self._device_image(img_a), self._device_image(img_b),
+                                                                   shape_a, shape_b)
+            return corr_a.cpu().numpy(), con_a.cpu().numpy(), None, corr_b.cpu().numpy(), con_b.cpu().numpy(), None
+        corr_a, con_a, corr_b, con_b = cotr_flow_maps(self.model, stretch_to_square_np(img_a.copy()), stretch_to_square_np(img_b.copy()))
+        resize = utils.float_image_resize
+        return resize(corr_a, shape_a), resize(con_a, shape_a), None, resize(corr_b, shape_b), resize(con_b, shape_b), None
 
     def gen_tasks(self, img_a, img_b, zoom_ins=[1.0], converge_iters=1, max_corrs=1000, queries_a=None, force=False, areas=None):
         if areas is not None:

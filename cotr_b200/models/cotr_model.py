@@ -397,6 +397,18 @@ class COTR(nn.Module):
         (inference_helper.py:155-160, :61-75): see cotr_flow_tile_merge in include/cotr_b200.h."""
         self.native().flow_tile_merge(tile, affine, patch, flow, conf, first)
 
+    @torch.no_grad()
+    def resize_image(self, img_u8, size):
+        """Device-side `PIL.Image.fromarray(img).resize((W', H'), BILINEAR)`: (H,W,3) uint8 CUDA image -> (H',W',3) uint8,
+        bit for bit (cotr_resize_image in include/cotr_b200.h).  size = (H', W')."""
+        return self.native().resize_image(img_u8, size)
+
+    @torch.no_grad()
+    def resize_maps(self, maps, size):
+        """Device-side `utils.float_image_resize`: (H,W) or (H,W,C) fp32 CUDA maps, C = 1 .. 3 -> size = (H', W'), bit for
+        bit (cotr_resize_maps in include/cotr_b200.h)."""
+        return self.native().resize_maps(maps, size)
+
     def _context(self, batch, reuse):
         nat = self.native()
         if reuse:

@@ -274,6 +274,30 @@ int cotr_dense_first_guess(int device, const float* flow_dev, const float* conf_
                            int h_to, int w_to, const void* kpts_dev, int kpt_is_f32, int n, double* loc_to_dev, int64_t* counts_dev,
                            void* cuda_stream);
 
+/* cotr_dense_first_guess on float32 maps: the same branch with the dtype rule of 'stretching' mode, where gen_tasks
+ * receives the maps from utils.float_image_resize as float32 whenever an image of the pair was stretched, bit for bit:
+ *   counts_dev[0] / [1] = #pixels with conf < 0.02f, compared in float32 (float32(0.02) is NOT counted; NaN is not).
+ *   loc_to_dev[i] = (double)(flow[r, c] * 0.5f + 0.5f) * (w_to, h_to): the scale and offset in float32 with separate
+ *   multiply and add, then one fp64 multiply by the int64 image size (numpy's promotion).
+ * Arguments, checks, pixel choice and launches as cotr_dense_first_guess. */
+int cotr_dense_first_guess_f32(int device, const float* flow_dev, const float* conf_from_dev, int h_from, int w_from,
+                               const float* conf_to_dev, int h_to, int w_to, const void* kpts_dev, int kpt_is_f32, int n, double* loc_to_dev,
+                               int64_t* counts_dev, void* cuda_stream);
+
+/* Whole-image resizes with Pillow's bilinear filter, bit for bit, on the device (what 'stretching' mode does on the host:
+ * stretch_to_square_np and utils.float_image_resize).  An axis whose size does not change is not resampled, as in Pillow
+ * (an identity pass would turn a NaN or infinite neighbour into NaN); with neither changing the output is a copy.
+ *   cotr_resize_image: src_dev h x w x 3 uint8 (RGB, HWC) -> dst_dev out_h x out_w x 3 uint8, equal to
+ *     PIL.Image.fromarray(src).resize((out_w, out_h), BILINEAR): 22-bit fixed-point tables, horizontal pass first with
+ *     uint8 rounding and clipping in between.
+ *   cotr_resize_maps: src_dev h x w x c fp32 (c = 1 .. 3, channels interleaved) -> dst_dev out_h x out_w x c fp32, equal to
+ *     utils.float_image_resize (Pillow mode 'F' per channel): double coefficients and accumulation, float32 after each pass.
+ * All sizes 1 .. 65536; src and dst DEVICE memory that must not overlap (maps 4-byte aligned).  Every argument is checked
+ * before anything is enqueued.  The coefficient tables (per input and output size, built and uploaded on first use) and
+ * the intermediate buffer are model-owned; once sizes have been seen, a call enqueues at most two kernels and never waits. */
+int cotr_resize_image(cotr_model* m, const uint8_t* src_dev, int h, int w, uint8_t* dst_dev, int out_h, int out_w, void* cuda_stream);
+int cotr_resize_maps(cotr_model* m, const float* src_dev, int h, int w, int c, float* dst_dev, int out_h, int out_w, void* cuda_stream);
+
 /* Squad formation of the grouped scheduler (FasterSparseEngine.form_grouped_batch / form_squad,
  * COTR/inference/sparse_engine.py:295-369) on the device.  pts_dev: n x 4 fp64 [x_from, y_from, x_to, y_to] of the open
  * tasks of one zoom level in the engine's (already shuffled) order; box_dev: n x 8 fp64, the central-half boxes
@@ -342,10 +366,11 @@ int cotr_last_launch_count(const cotr_model* m);
  * (the maps of cotr_*_attention), 11 match_queries, 12 match_pixels, 13 nearest, 14 mutual (cotr_match_keypoints),
  * 15 refine_geometry, 16 resize_h, 17 resize_v, 18 refine_step (cotr_refine and cotr_refine_grouped),
  * 19 grouped_candidates, 20 group_tasks (cotr_refine_grouped), 21 dense_first_guess (reserved: cotr_dense_first_guess
- * takes no model, so its launch has no profiler to record it).  For GEMMs M,N,K are the problem size; for attention and
+ * takes no model, so its launch has no profiler to record it), 22 resize_image (cotr_resize_image), 23 resize_maps
+ * (cotr_resize_maps).  For GEMMs M,N,K are the problem size; for attention and
  * attention weights M = query rows, N = 512, K = 256; for 11-13 M = rows, N = 2; for 14 M = pairs; for 15 and 18
  * M = tasks of the launch (cotr_refine_grouped: its candidates), N = level; for 16-17 M = crops; for 19-20
- * M = candidates, N = level. */
+ * M = candidates, N = level; for 22-23 M = output rows of the pass, N = output columns, K = 0 horizontal / 1 vertical. */
 typedef struct cotr_launch_record {
     int32_t kernel;
     int32_t M, N, K;
